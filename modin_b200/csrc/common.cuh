@@ -62,10 +62,37 @@ __device__ __forceinline__ uint64_t l2_policy_evict_first() {
   return pol;
 }
 
-// Four-element tiles, moved as two 128-bit accesses (LDG.E.128 / STG.E.128 on sm_90a).
 // Deliberately NOT `.nc`: ptxas sinks non-coherent loads below independent stores to save
 // registers, which serialises the unrolled loads; plain ld.global keeps every load of a
 // tile ahead of the first store.
+//
+// Two-element pairs, one 128-bit access each (LDG.E.128 / STG.E.128 on sm_90a).  With lane i
+// at p + 2 i, one warp instruction covers 512 contiguous bytes: 16 whole 32-byte sectors.
+__device__ __forceinline__ double2 ldg_stream_f64x2(const double* p) {
+  double2 v;
+  asm volatile("ld.global.L1::no_allocate.L2::cache_hint.v2.f64 {%0,%1}, [%2], %3;"
+               : "=d"(v.x), "=d"(v.y)
+               : "l"(p), "l"(l2_policy_evict_first()));
+  return v;
+}
+__device__ __forceinline__ longlong2 ldg_stream_i64x2(const long long* p) {
+  longlong2 v;
+  asm volatile("ld.global.L1::no_allocate.L2::cache_hint.v2.s64 {%0,%1}, [%2], %3;"
+               : "=l"(v.x), "=l"(v.y)
+               : "l"(p), "l"(l2_policy_evict_first()));
+  return v;
+}
+__device__ __forceinline__ void stg_stream_f64x2(double* p, const double2& v) {
+  asm volatile("st.global.L1::no_allocate.v2.f64 [%0], {%1,%2};" ::"l"(p), "d"(v.x), "d"(v.y) : "memory");
+}
+__device__ __forceinline__ void stg_stream_i64x2(long long* p, const longlong2& v) {
+  asm volatile("st.global.L1::no_allocate.v2.s64 [%0], {%1,%2};" ::"l"(p), "l"(v.x), "l"(v.y) : "memory");
+}
+
+// Four-element tiles, moved as two 128-bit accesses 16 B apart, at p and p + 2.  Lane i at p + 4 i
+// therefore uses half of every sector per warp instruction; only reduce_ldg_kernel and
+// key_range_kernel use these, because which element a lane reads fixes their summation order and
+// their key sample.
 struct __align__(32) f64x4 {
   double x, y, z, w;
 };
@@ -92,20 +119,6 @@ __device__ __forceinline__ i64x4 ldg_stream_i64x4(const long long* p) {
       : "=l"(v.x), "=l"(v.y), "=l"(v.z), "=l"(v.w)
       : "l"(p), "l"(p + 2), "l"(pol));
   return v;
-}
-__device__ __forceinline__ void stg_stream_f64x4(double* p, const f64x4& v) {
-  asm volatile(
-      "st.global.L1::no_allocate.v2.f64 [%0], {%2,%3};\n\t"
-      "st.global.L1::no_allocate.v2.f64 [%1], {%4,%5};" ::"l"(p),
-      "l"(p + 2), "d"(v.x), "d"(v.y), "d"(v.z), "d"(v.w)
-      : "memory");
-}
-__device__ __forceinline__ void stg_stream_i64x4(long long* p, const i64x4& v) {
-  asm volatile(
-      "st.global.L1::no_allocate.v2.s64 [%0], {%2,%3};\n\t"
-      "st.global.L1::no_allocate.v2.s64 [%1], {%4,%5};" ::"l"(p),
-      "l"(p + 2), "l"(v.x), "l"(v.y), "l"(v.z), "l"(v.w)
-      : "memory");
 }
 // Scalar streaming loads take the same cache-policy operand.
 __device__ __forceinline__ uint64_t l2_policy_evict_last() {

@@ -1,10 +1,11 @@
 // elementwise.cu — Map / Binary operator templates as coalesced 128-bit column sweeps.
 //
-// One launch covers every column of a block (Modin partition): a persistent grid of
-// (SM count x resident CTAs) walks (column, row-tile) pairs.  Each thread moves 4 four-element
-// vectors (two 128-bit accesses each) per operand per tile, all loads issued before the first use
-// (LDG.E.128, L1 bypass, L2 evict-first), results stored with STG.E.128.  The path is HBM-bound: algorithmic traffic
-// is 8 B read per operand element + 8 B written (1 B for predicates).
+// One launch covers every column of a block (Modin partition): one CTA per (4096-row tile, column).
+// The tile is 8 slabs of 512 rows; in each slab thread t moves rows 2t and 2t + 1 with one access
+// per operand (LDG.E.128 / STG.E.128 for 8-byte types, 16-bit for bool columns), so every warp
+// instruction covers whole contiguous sectors.  All loads of a tile are issued before the first
+// store (L1 bypass, L2 evict-first).  The path is HBM-bound: algorithmic traffic is 8 B read per
+// operand element + 8 B written (1 B for predicates).
 //
 // pandas semantics restated here (reference call sites):
 //   abs/neg/isna/notna  Map.register(pandas.DataFrame.abs ...)   qc.py:2036, 2063-2106
@@ -20,9 +21,10 @@
 namespace mb200 {
 
 constexpr int kThreads = 256;
-constexpr int kUnroll = 4;
-constexpr int kVec = 4;
-constexpr int kTile = kThreads * kUnroll * kVec;  // 4096 elements = 32 KiB of f64 per operand
+constexpr int kPair = 2;                  // elements per thread and access
+constexpr int kSlab = kThreads * kPair;   // 512 elements
+constexpr int kSlabs = 8;
+constexpr int kTile = kSlab * kSlabs;     // 4096 elements = 32 KiB of f64 per operand
 
 struct MapParams {
   const void* in0[MB200_MAX_COLS];
@@ -31,9 +33,7 @@ struct MapParams {
   void* out[MB200_MAX_COLS];
   uint64_t s0[MB200_MAX_COLS];
   uint64_t s1[MB200_MAX_COLS];
-  int ncols;
   long long nrows;
-  long long tiles_per_col;
 };
 
 template <typename T>
@@ -156,146 +156,82 @@ __device__ __forceinline__ TO apply(TI a, TI b, TI c, TI s0, TI s1) {
   }
 }
 
+// One element pair per thread and slab: a 16-byte access for the 8-byte types, 2 bytes for bool (uint8) columns.
 template <typename T>
-struct Vec4;
+struct Pair;
 template <>
-struct Vec4<double> {
-  using type = f64x4;
-  static __device__ __forceinline__ f64x4 load(const double* p) { return ldg_stream_f64x4(p); }
-  static __device__ __forceinline__ void store(double* p, const f64x4& v) { stg_stream_f64x4(p, v); }
+struct Pair<double> {
+  using type = double2;
+  static __device__ __forceinline__ double2 load(const double* p) { return ldg_stream_f64x2(p); }
+  static __device__ __forceinline__ void store(double* p, const double2& v) { stg_stream_f64x2(p, v); }
 };
 template <>
-struct Vec4<long long> {
-  using type = i64x4;
-  static __device__ __forceinline__ i64x4 load(const long long* p) { return ldg_stream_i64x4(p); }
-  static __device__ __forceinline__ void store(long long* p, const i64x4& v) { stg_stream_i64x4(p, v); }
-};
-
-// bool columns (uint8 0 / 1): four elements = one 32-bit word
-struct u8x4 {
-  uint8_t x, y, z, w;
+struct Pair<long long> {
+  using type = longlong2;
+  static __device__ __forceinline__ longlong2 load(const long long* p) { return ldg_stream_i64x2(p); }
+  static __device__ __forceinline__ void store(long long* p, const longlong2& v) { stg_stream_i64x2(p, v); }
 };
 template <>
-struct Vec4<uint8_t> {
-  using type = u8x4;
-  static __device__ __forceinline__ u8x4 load(const uint8_t* p) {
-    const uint32_t v = __ldg(reinterpret_cast<const uint32_t*>(p));
-    u8x4 r;
-    r.x = (uint8_t)(v & 0xffu);
-    r.y = (uint8_t)((v >> 8) & 0xffu);
-    r.z = (uint8_t)((v >> 16) & 0xffu);
-    r.w = (uint8_t)(v >> 24);
-    return r;
-  }
+struct Pair<uint8_t> {
+  using type = uchar2;
+  static __device__ __forceinline__ uchar2 load(const uint8_t* p) { return __ldg(reinterpret_cast<const uchar2*>(p)); }
+  static __device__ __forceinline__ void store(uint8_t* p, const uchar2& v) { *reinterpret_cast<uchar2*>(p) = v; }
 };
 
-template <typename TO, typename VO>
-__device__ __forceinline__ void store_out(TO* p, const VO& v) {
-  if constexpr (sizeof(TO) == 1) {
-    uint32_t packed = (uint32_t)v.x | ((uint32_t)v.y << 8) | ((uint32_t)v.z << 16) | ((uint32_t)v.w << 24);
-    *reinterpret_cast<uint32_t*>(p) = packed;
-  } else {
-    Vec4<TO>::store(p, v);
-  }
-}
-template <typename TO>
-struct OutVec {
-  TO x, y, z, w;
-};
-template <>
-struct OutVec<double> : f64x4 {};
-template <>
-struct OutVec<long long> : i64x4 {};
-
-// VEC=true: every operand pointer is 32-byte aligned -> vector path; else scalar sweep.
+// VEC=true: every operand pointer is 16-byte aligned -> vector path; else scalar sweep.
 template <int OP, typename TI, typename TO, bool VEC>
 __global__ void __launch_bounds__(kThreads) map_kernel(const __grid_constant__ MapParams p) {
   constexpr int NIN = op_nin(OP);
-  const long long ntiles = p.tiles_per_col * p.ncols;
   const int tid = threadIdx.x;
-  for (long long t = blockIdx.x; t < ntiles; t += gridDim.x) {
-    const int col = (int)(t / p.tiles_per_col);
-    const long long base = (t - (long long)col * p.tiles_per_col) * kTile;
-    const TI* __restrict__ a = static_cast<const TI*>(p.in0[col]);
-    const TI* __restrict__ b = NIN >= 2 ? static_cast<const TI*>(p.in1[col]) : nullptr;
-    const TI* __restrict__ c = NIN >= 3 ? static_cast<const TI*>(p.in2[col]) : nullptr;
-    TO* __restrict__ o = static_cast<TO*>(p.out[col]);
-    const TI s0 = from_bits<TI>(p.s0[col]);
-    const TI s1 = from_bits<TI>(p.s1[col]);
-    if (VEC && base + kTile <= p.nrows) {
-      using V = typename Vec4<TI>::type;
-      V va[kUnroll], vb[kUnroll], vc[kUnroll];
+  // one CTA per (row tile, column), as the Fold kernels: no per-tile index arithmetic, no tile loop
+  const int col = blockIdx.y;
+  const long long base = (long long)blockIdx.x * kTile;
+  const TI* __restrict__ a = static_cast<const TI*>(p.in0[col]);
+  const TI* __restrict__ b = NIN >= 2 ? static_cast<const TI*>(p.in1[col]) : nullptr;
+  const TI* __restrict__ c = NIN >= 3 ? static_cast<const TI*>(p.in2[col]) : nullptr;
+  TO* __restrict__ o = static_cast<TO*>(p.out[col]);
+  const TI s0 = from_bits<TI>(p.s0[col]);
+  const TI s1 = from_bits<TI>(p.s1[col]);
+  if (VEC && base + kTile <= p.nrows) {
+    // slab k, thread t: elements base + k * kSlab + 2 t and + 1, so each warp instruction covers whole sectors
+    typename Pair<TI>::type va[kSlabs], vb[kSlabs], vc[kSlabs];
 #pragma unroll
-      for (int u = 0; u < kUnroll; ++u) {
-        const long long i = base + (long long)(u * kThreads + tid) * kVec;
-        va[u] = Vec4<TI>::load(a + i);
-        if constexpr (NIN >= 2) vb[u] = Vec4<TI>::load(b + i);
-        if constexpr (NIN >= 3) vc[u] = Vec4<TI>::load(c + i);
-      }
+    for (int k = 0; k < kSlabs; ++k) {
+      const long long i = base + k * kSlab + kPair * tid;
+      va[k] = Pair<TI>::load(a + i);
+      if constexpr (NIN >= 2) vb[k] = Pair<TI>::load(b + i);
+      if constexpr (NIN >= 3) vc[k] = Pair<TI>::load(c + i);
+    }
 #pragma unroll
-      for (int u = 0; u < kUnroll; ++u) {
-        const long long i = base + (long long)(u * kThreads + tid) * kVec;
-        OutVec<TO> r;
-        if constexpr (NIN == 1) {
-          r.x = apply<OP, TI, TO>(va[u].x, 0, 0, s0, s1);
-          r.y = apply<OP, TI, TO>(va[u].y, 0, 0, s0, s1);
-          r.z = apply<OP, TI, TO>(va[u].z, 0, 0, s0, s1);
-          r.w = apply<OP, TI, TO>(va[u].w, 0, 0, s0, s1);
-        } else if constexpr (NIN == 2) {
-          r.x = apply<OP, TI, TO>(va[u].x, vb[u].x, 0, s0, s1);
-          r.y = apply<OP, TI, TO>(va[u].y, vb[u].y, 0, s0, s1);
-          r.z = apply<OP, TI, TO>(va[u].z, vb[u].z, 0, s0, s1);
-          r.w = apply<OP, TI, TO>(va[u].w, vb[u].w, 0, s0, s1);
-        } else {
-          r.x = apply<OP, TI, TO>(va[u].x, vb[u].x, vc[u].x, s0, s1);
-          r.y = apply<OP, TI, TO>(va[u].y, vb[u].y, vc[u].y, s0, s1);
-          r.z = apply<OP, TI, TO>(va[u].z, vb[u].z, vc[u].z, s0, s1);
-          r.w = apply<OP, TI, TO>(va[u].w, vb[u].w, vc[u].w, s0, s1);
-        }
-        store_out<TO>(o + i, r);
-      }
-    } else {
-      const long long end = (base + kTile < p.nrows) ? base + kTile : p.nrows;
-      for (long long i = base + tid; i < end; i += kThreads) {
-        TI x = a[i];
-        TI y = NIN >= 2 ? b[i] : (TI)0;
-        TI z = NIN >= 3 ? c[i] : (TI)0;
-        o[i] = apply<OP, TI, TO>(x, y, z, s0, s1);
-      }
+    for (int k = 0; k < kSlabs; ++k) {
+      const long long i = base + k * kSlab + kPair * tid;
+      TI bx = 0, by = 0, cx = 0, cy = 0;
+      if constexpr (NIN >= 2) bx = vb[k].x, by = vb[k].y;
+      if constexpr (NIN >= 3) cx = vc[k].x, cy = vc[k].y;
+      typename Pair<TO>::type r;
+      r.x = apply<OP, TI, TO>(va[k].x, bx, cx, s0, s1);
+      r.y = apply<OP, TI, TO>(va[k].y, by, cy, s0, s1);
+      Pair<TO>::store(o + i, r);
+    }
+  } else {
+    const long long end = (base + kTile < p.nrows) ? base + kTile : p.nrows;
+    for (long long i = base + tid; i < end; i += kThreads) {
+      TI x = a[i];
+      TI y = NIN >= 2 ? b[i] : (TI)0;
+      TI z = NIN >= 3 ? c[i] : (TI)0;
+      o[i] = apply<OP, TI, TO>(x, y, z, s0, s1);
     }
   }
 }
 
-template <int OP, typename TI, typename TO>
-static int launch_map(const MapParams& p, bool vec, int grid, cudaStream_t st) {
-  if (vec)
-    map_kernel<OP, TI, TO, true><<<grid, kThreads, 0, st>>>(p);
-  else
-    map_kernel<OP, TI, TO, false><<<grid, kThreads, 0, st>>>(p);
-  MB_LAUNCH_CHECK("map_kernel");
-  return 0;
-}
-
-template <int OP, typename TI, typename TO>
-static int grid_for(int* grid, long long ntiles) {
-  DevProps dp;
-  if (int rc = dev_props(&dp)) return rc;
-  int occ = 0;
-  MB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, map_kernel<OP, TI, TO, true>, kThreads, 0));
-  if (occ < 1) occ = 1;
-  long long g = (long long)dp.sm_count * occ;  // one full wave of resident CTAs, persistent loop
-  if (g > ntiles) g = ntiles;
-  if (g < 1) g = 1;
-  *grid = (int)g;
-  return 0;
-}
-
-#define MB_CASE(OPC, TI, TO)                                              \
-  case OPC: {                                                             \
-    int grid;                                                             \
-    if (int rc = grid_for<OPC, TI, TO>(&grid, ntiles)) return rc;         \
-    return launch_map<OPC, TI, TO>(p, vec, grid, st);                     \
-  }
+#define MB_CASE(OPC, TI, TO)                                     \
+  case OPC:                                                      \
+    if (vec)                                                     \
+      map_kernel<OPC, TI, TO, true><<<grid, kThreads, 0, st>>>(p);  \
+    else                                                         \
+      map_kernel<OPC, TI, TO, false><<<grid, kThreads, 0, st>>>(p); \
+    MB_LAUNCH_CHECK("map_kernel");                               \
+    return 0;
 
 }  // namespace mb200
 
@@ -322,15 +258,15 @@ extern "C" int mb200_map(int op, int dtype, int ncols, const void* const* in0, c
     p.s0[c] = s0 ? s0[c] : 0;
     p.s1[c] = s1 ? s1[c] : 0;
     if (!in0[c] || !out[c]) return fail("mb200_map", "null column pointer");
-    vec = vec && aligned32(in0[c]) && aligned32(out[c]);
-    if (nin >= 2) vec = vec && in1[c] && aligned32(in1[c]);
-    if (nin >= 3) vec = vec && in2[c] && aligned32(in2[c]);
+    vec = vec && aligned16(in0[c]) && aligned16(out[c]);
+    if (nin >= 2) vec = vec && in1[c] && aligned16(in1[c]);
+    if (nin >= 3) vec = vec && in2[c] && aligned16(in2[c]);
     if ((nin >= 2 && !in1[c]) || (nin >= 3 && !in2[c])) return fail("mb200_map", "null column pointer");
   }
-  p.ncols = ncols;
   p.nrows = nrows;
-  p.tiles_per_col = (nrows + kTile - 1) / kTile;
-  const long long ntiles = p.tiles_per_col * ncols;
+  const long long tiles_per_col = (nrows + kTile - 1) / kTile;
+  if (tiles_per_col > 0x7fffffffLL) return fail("mb200_map", "too many rows for one launch");
+  const dim3 grid((unsigned)tiles_per_col, (unsigned)ncols);
   cudaStream_t st = (cudaStream_t)stream;
 
   if (dtype == MB200_F64) {
