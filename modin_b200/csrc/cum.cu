@@ -7,7 +7,7 @@
 // ignores them and the output keeps NaN where the input had it (nanops / masked_accumulations: fill with the identity,
 // accumulate, restore).  That is a scan over a monoid, so it parallelises:
 //
-//   value v[i]  = identity where x[i] is NaN, else x[i]
+//   value v[i]  = identity where x[i] is NaN (+0.0 for the sum, whose identity is -0.0), else x[i]
 //   S[i]        = v[0] (+) ... (+) v[i]            (+) in {+, max, min, "latest valid"}
 //   out[i]      = NaN where x[i] is NaN, else S[i]  (forward fill: S[i] everywhere)
 //
@@ -47,7 +47,7 @@ struct CumT<double> {
   static __device__ __forceinline__ bool skip(double x) { return x != x; }
   template <int OP>
   static __device__ __forceinline__ double ident() {
-    if (OP == MB200_CUM_SUM) return 0.0;
+    if (OP == MB200_CUM_SUM) return __longlong_as_double(0x8000000000000000LL);  // -0.0: x + -0.0 = x for every x
     if (OP == MB200_CUM_MAX) return __longlong_as_double(0xfff0000000000000LL);  // -inf
     if (OP == MB200_CUM_MIN) return __longlong_as_double(0x7ff0000000000000LL);  // +inf
     return __longlong_as_double(0x7ff8000000000000LL);                           // FFILL: NaN = "nothing valid yet"
@@ -68,9 +68,20 @@ struct CumT<long long> {
 template <int OP, typename T>
 __device__ __forceinline__ T cum_comb(T a, T b) {
   if (OP == MB200_CUM_SUM) return a + b;
-  if (OP == MB200_CUM_MAX) return b > a ? b : a;
-  if (OP == MB200_CUM_MIN) return b < a ? b : a;
+  // ties go to the later operand: pandas' cummax / cummin (numpy's maximum / minimum.accumulate) return the latest
+  // of equal values, which tells -0.0 from 0.0
+  if (OP == MB200_CUM_MAX) return b >= a ? b : a;
+  if (OP == MB200_CUM_MIN) return b <= a ? b : a;
   return CumT<T>::skip(b) ? a : b;  // FFILL: the latest valid value
+}
+
+// the running value after a row: NaN rows leave max / min / forward fill as they were and add +0.0 to a sum.  pandas
+// fills NaN with 0.0 and accumulates from the first row, so cumsum([-0.0]) = [-0.0] (hence the identity -0.0) but
+// cumsum([NaN, -0.0]) = [NaN, +0.0]
+template <int OP, typename T>
+__device__ __forceinline__ T cum_step(T run, T v) {
+  if (!CumT<T>::skip(v)) return cum_comb<OP, T>(run, v);
+  return OP == MB200_CUM_SUM ? cum_comb<OP, T>(run, (T)0) : run;
 }
 
 __device__ __forceinline__ int cum_slot(int j) { return j + (j >> 4); }
@@ -100,8 +111,7 @@ __global__ void __launch_bounds__(kCumBlock) cum_tile_reduce_kernel(const __grid
   const int s0 = (int)threadIdx.x * (kCumPer + 1);  // cum_slot(16 t + k) = 17 t + k
 #pragma unroll
   for (int k = 0; k < kCumPer; ++k) {
-    const T v = tile[s0 + k];
-    if (!CumT<T>::skip(v)) acc = cum_comb<OP, T>(acc, v);
+    acc = cum_step<OP, T>(acc, tile[s0 + k]);
   }
   // ordered tree: after the step with distance m, lane i holds rows of lanes [i, i + 2m)
 #pragma unroll
@@ -168,7 +178,7 @@ __global__ void __launch_bounds__(kCumBlock) cum_tile_scan_kernel(const __grid_c
 #pragma unroll
   for (int k = 0; k < kCumPer; ++k) {
     v[k] = tile[s0 + k];
-    if (!CumT<T>::skip(v[k])) tot = cum_comb<OP, T>(tot, v[k]);
+    tot = cum_step<OP, T>(tot, v[k]);
   }
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   T incl = tot;
@@ -186,9 +196,8 @@ __global__ void __launch_bounds__(kCumBlock) cum_tile_scan_kernel(const __grid_c
   if (lane > 0) run = cum_comb<OP, T>(run, prev);
 #pragma unroll
   for (int k = 0; k < kCumPer; ++k) {
-    const bool nan = CumT<T>::skip(v[k]);
-    if (!nan) run = cum_comb<OP, T>(run, v[k]);
-    tile[s0 + k] = (nan && OP != MB200_CUM_FFILL) ? v[k] : run;
+    run = cum_step<OP, T>(run, v[k]);
+    tile[s0 + k] = (CumT<T>::skip(v[k]) && OP != MB200_CUM_FFILL) ? v[k] : run;
   }
   __syncthreads();
 #pragma unroll

@@ -12,7 +12,8 @@
 //       block reduction;
 //   variant 1: direct 128-bit streaming loads (LDG.E.128), same reduction tree.
 // Per-thread float sums are Kahan-compensated (error O(eps)*sum|x| independent of n; the
-// compensation is reset when it becomes NaN so +-inf inputs behave like pandas/numpy).
+// compensation is dropped while the running sum is not finite, so +-inf inputs and sums that
+// overflow to +-inf behave like pandas/numpy).
 // Stage 2 (reduce_finalize) combines the per-CTA partials in fixed order.
 // Algorithmic traffic: 8 B read per element; output ncols * 16 B.
 #include <math.h>
@@ -56,8 +57,9 @@ struct Acc<MB200_RED_SUM, double> {
     const double v = (ok || !skipna) ? x : 0.0;
     const double y = v - c;
     const double t = s + y;
-    double cc = (t - s) - y;
-    c = (cc != cc) ? 0.0 : cc;  // inf - inf: drop the compensation, keep the running sum
+    // a running sum that is +-inf (an inf input, or overflow) or NaN carries no compensation: (t - s) - y would be
+    // inf or NaN, and value() = s - c would turn an overflowed sum into inf - inf = NaN
+    c = isfinite(t) ? (t - s) - y : 0.0;
     s = t;
   }
   __device__ __forceinline__ void merge(const Acc& o) {
@@ -68,8 +70,7 @@ struct Acc<MB200_RED_SUM, double> {
   __device__ __forceinline__ void add_raw(double v) {
     const double y = v - c;
     const double t = s + y;
-    double cc = (t - s) - y;
-    c = (cc != cc) ? 0.0 : cc;
+    c = isfinite(t) ? (t - s) - y : 0.0;
     s = t;
   }
   __device__ __forceinline__ double value() const { return s - c; }

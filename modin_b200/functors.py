@@ -1128,9 +1128,12 @@ class DevReindex(DevFn):
             src = block.index_cols[0] if block.index_cols else ops.iota(block.range_start, block.nrows)
             tgt_np = labels.to_numpy()
             if src.dtype == np.float64 or tgt_np.dtype.kind == "f":
-                # float labels (or int against float): compare through the order-preserving int64 image
-                tgt = ops.map_columns("ordered_s", [DeviceColumn.from_numpy(tgt_np.astype(np.float64))], s0=[0])[0]
-                src = ops.map_columns("ordered_s", ops.cast_columns_f64([src]), s0=[0])[0]
+                # float labels (or int against float): compare through the order-preserving int64 image, in which
+                # -0.0 and 0.0 are one label
+                from .groupkeys import float_image
+
+                tgt = float_image(DeviceColumn.from_numpy(tgt_np.astype(np.float64)))
+                src = float_image(ops.cast_columns_f64([src])[0])
             else:
                 tgt = DeviceColumn.from_numpy(tgt_np.astype(np.int64))
             table = ops.JoinTable(src)

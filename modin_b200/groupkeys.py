@@ -81,7 +81,14 @@ def float_image(key: DeviceColumn) -> DeviceColumn:
         raise TypeError("float_image takes a float64 column")
     if not len(key):
         return DeviceColumn.empty(0, np.int64)
-    return ops.map_columns("ordered_s", ops.map_columns("add_s", [key], s0=[0.0]), s0=[0])[0]
+    return ops.map_columns("ordered_s", [fold_zero_sign(key)], s0=[0])[0]
+
+
+def fold_zero_sign(key: DeviceColumn) -> DeviceColumn:
+    """``key + 0.0``: ``-0.0`` becomes ``0.0``, every other value is unchanged (NaN stays NaN).  pandas treats the
+    two zeros as one key when it groups, sorts (ties, kept in row order) and matches labels, so every order-preserving
+    image of a float64 key is taken from this column, never from the raw bits."""
+    return ops.map_columns("add_s", [key], s0=[0.0])[0]
 
 
 def float_keys(image: DeviceColumn) -> np.ndarray:

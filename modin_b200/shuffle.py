@@ -28,6 +28,7 @@ import numpy as np
 from . import dist, ops
 from .block import DeviceBlock, DeviceColumn, concat_rows
 from .functors import DevFn, _check_block
+from .groupkeys import fold_zero_sign
 
 
 def _with_label_column(block: DeviceBlock) -> DeviceBlock:
@@ -49,8 +50,9 @@ def key_image(block: DeviceBlock, key_position: int, ascending: bool) -> DeviceC
         raise NotImplementedError("device range partitioning needs a float64 or int64 key column")
     if block.nrows == 0:
         return DeviceColumn.empty(0, np.int64)
-    desc = (1.0 if key.dtype == np.float64 else 1) if not ascending else 0
-    return ops.map_columns("ordered_s", [key], s0=[desc])[0]
+    if key.dtype == np.float64:  # -0.0 and 0.0 tie: rows keep their order, as in pandas' stable sort
+        return ops.map_columns("ordered_s", [fold_zero_sign(key)], s0=[0.0 if ascending else 1.0])[0]
+    return ops.map_columns("ordered_s", [key], s0=[0 if ascending else 1])[0]
 
 
 class DevShuffleFunctions:

@@ -362,16 +362,16 @@ def concat_columns(pieces):
     return pieces[0] if len(pieces) == 1 else _col(np.concatenate([_np(p) for p in pieces]))
 
 
-_CUM_ID = {"sum": 0.0, "max": -np.inf, "min": np.inf, "ffill": np.nan}
+_CUM_ID = {"sum": -0.0, "max": -np.inf, "min": np.inf, "ffill": np.nan}  # -0.0: x + -0.0 = x (csrc/cum.cu)
 
 
 def _cum_comb(op, a, b):
     if op == "sum":
         return a + b
-    if op == "max":
-        return np.maximum(a, b)
+    if op == "max":  # ties go to the later operand, b
+        return np.where(b >= a, b, a)
     if op == "min":
-        return np.minimum(a, b)
+        return np.where(b <= a, b, a)
     return np.where(np.isnan(b), a, b)
 
 
@@ -394,9 +394,12 @@ def cum_partials(op, cols):
         for j in idxs:
             x = _np(cols[j])
             v = x[~np.isnan(x)] if x.dtype == np.float64 else x
+            if op == "sum" and x.dtype == np.float64:
+                v = np.where(np.isnan(x), 0.0, x)  # NaN rows add +0.0
             ident = _cum_ident(op, x.dtype)
             with np.errstate(all="ignore"):
-                tot.append(ident if len(v) == 0 else {"sum": v.sum, "max": v.max, "min": v.min, "ffill": lambda: v[-1]}[op]())
+                tot.append(ident if len(v) == 0 else {"sum": lambda: np.cumsum(v)[-1], "max": v.max, "min": v.min,
+                                                     "ffill": lambda: v[-1]}[op]())  # cumsum: -0.0 + -0.0 stays -0.0
         st.groups.append((code, idxs, None, torch.from_numpy(np.asarray(tot, dtype=_np(cols[idxs[0]]).dtype))))
     return st
 
@@ -427,7 +430,7 @@ def cum_apply(state, cols, carries=None):
                     r = pandas.Series(x).ffill().to_numpy()
                     r = np.where(np.isnan(r), carry, r)
                 else:
-                    v = np.where(nan, ident, x)
+                    v = np.where(nan, 0.0 if op == "sum" else ident, x)
                     acc = {"sum": np.cumsum, "max": np.maximum.accumulate, "min": np.minimum.accumulate}[op](v)
                     r = _cum_comb(op, np.full(len(x), carry, dtype=x.dtype), acc).astype(x.dtype)
                     if x.dtype == np.float64:

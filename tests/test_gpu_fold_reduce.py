@@ -18,6 +18,7 @@ import pandas
 import pytest
 
 from modin_b200 import synth
+from tests.exact import assert_bits
 
 pytestmark = pytest.mark.gpu
 
@@ -40,7 +41,7 @@ def _check(op, got, x):
         ok = np.isnan(want) | (np.abs(got - want) <= bound)
         assert ok.all(), (op, len(x), int((~ok).sum()))
     else:
-        assert np.array_equal(got, want, equal_nan=True), (op, len(x))
+        assert_bits(got, want, f"cum{op} n={len(x)}")
 
 
 def _host_columns(n, seed):

@@ -9,7 +9,6 @@ BIT-EXACT (NaN == NaN); float sums and means satisfy
 """
 
 import glob
-import math
 import os
 
 import numpy as np
@@ -18,10 +17,9 @@ import pytest
 
 from modin_b200 import synth
 from oracle import reference_path as orc
+from tests.exact import EPS, assert_exact, assert_sum_close, assert_within_sum_bound, exact_group_sums
 
 pytestmark = pytest.mark.gpu
-
-EPS = 2.0**-53
 
 
 def bpd():
@@ -60,31 +58,6 @@ def _load(golden_dir, pattern):
     files = sorted(glob.glob(os.path.join(golden_dir, pattern)))
     assert files
     return [(os.path.basename(f), np.load(f, allow_pickle=False)) for f in files]
-
-
-def assert_exact(got, want, what):
-    got, want = np.asarray(got), np.asarray(want)
-    assert got.shape == want.shape, f"{what}: shape {got.shape} vs {want.shape}"
-    if want.dtype.kind == "f" or got.dtype.kind == "f":
-        g, w = got.astype(np.float64), want.astype(np.float64)
-        both_nan = np.isnan(g) & np.isnan(w)
-        same = (g.view(np.uint64) == w.view(np.uint64)) | both_nan
-        assert same.all(), f"{what}: {np.count_nonzero(~same)} elements differ (bit-exact, NaN==NaN)"
-    else:
-        assert np.array_equal(got, want), f"{what}: integer/bool mismatch"
-
-
-def sum_tolerance(abs_sum, n):
-    return 4.0 * max(1.0, math.log2(max(n, 2))) * EPS * abs_sum + 1e-300
-
-
-def assert_sum_close(got, want, abs_sums, n, what):
-    got, want = np.asarray(got, dtype=np.float64), np.asarray(want, dtype=np.float64)
-    assert got.shape == want.shape, f"{what}: shape"
-    tol = np.array([sum_tolerance(a, n) for a in np.asarray(abs_sums, dtype=np.float64).ravel()]).reshape(got.shape)
-    both_nan = np.isnan(got) & np.isnan(want)
-    ok = both_nan | (np.abs(got - want) <= tol) | (got == want)
-    assert ok.all(), f"{what}: max err {np.nanmax(np.abs(got - want))} vs tol {tol.max()}"
 
 
 # ---------------------------------------------------------------------------------------------
@@ -322,9 +295,15 @@ def test_groups_whose_rows_leave_no_trace_are_still_groups(gb_table_kind):
         assert_exact(got.index.to_numpy(), want.index.to_numpy(), f"{agg} keys")
         w = want.to_numpy(dtype=np.float64).reshape(len(want), -1)
         gt = got.to_numpy(dtype=np.float64).reshape(len(got), -1)
-        if agg in ("sum", "mean"):
+        if agg == "sum":
+            keys, exact = exact_group_sums(pdf["key"].to_numpy(), pdf[["c0", "c1", "c2"]].to_numpy())
+            assert_exact(keys, want.index.to_numpy(), "exact reference keys")
+            abs_by_group = pdf[["c0", "c1", "c2"]].abs().groupby(pdf["key"]).sum().to_numpy()
+            assert_within_sum_bound(gt, exact, abs_by_group, n, "groupby sum vs exact")
+            assert_exact(gt[np.isin(want.index.to_numpy(), [0, 6, 12])], w[np.isin(want.index.to_numpy(), [0, 6, 12])],
+                         "all-NaN / all -0.0 groups sum to +0.0")  # fmt: skip
+        elif agg == "mean":
             assert np.allclose(gt, w, rtol=0, atol=1e-9, equal_nan=True), agg
-            assert not np.signbit(gt[np.isin(want.index.to_numpy(), [0, 6, 12])]).any() or agg == "mean"
         else:
             assert_exact(gt, w, f"groupby {agg}")
 

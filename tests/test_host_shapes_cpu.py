@@ -305,6 +305,35 @@ def test_frames_whose_labels_are_not_a_plain_range(frames):
         ds[ds["c0"] > 0.0]._to_pandas()  # string labels cannot ride through the device compaction: refused, not dropped
 
 
+def test_sort_values_treats_the_two_zeros_as_a_tie(cpu_device):
+    """pandas sorts ``-0.0`` and ``0.0`` as a tie: rows keep their order.  The device sort key folds ``-0.0`` into
+    ``0.0`` before it orders the bits; the gathered values keep theirs."""
+    import modin_b200.pandas as bpd
+
+    x = np.array([0.0, -0.0, 1.0, -0.0, 0.0, np.nan, -1.0, -0.0, np.inf, 0.0, -np.inf] * 37)
+    pdf = pandas.DataFrame({"x": x, "v": np.arange(len(x), dtype=np.float64)})
+    df = bpd.DataFrame(pdf)
+    for asc in (True, False):
+        got = df.sort_values("x", ascending=asc)._to_pandas()
+        want = pdf.sort_values("x", ascending=asc, kind="stable")
+        assert list(got.index) == list(want.index), f"sort ascending={asc}: row order"
+        assert np.array_equal(got.to_numpy().view(np.int64), want.to_numpy().view(np.int64)), f"sort ascending={asc}: bits"
+
+
+def test_alignment_matches_a_negative_zero_label_to_zero(cpu_device):
+    """Frames with different float row labels are re-indexed onto the joined labels; pandas matches a ``-0.0`` label
+    in one frame to the ``0.0`` of the other."""
+    import modin_b200.pandas as bpd
+
+    a = pandas.DataFrame({"c": [1.0, 2.0, 4.0, 8.0]}, index=pandas.Index([0.0, 1.0, 2.0, 5.0]))
+    b = pandas.DataFrame({"c": [16.0, 32.0, 64.0]}, index=pandas.Index([-0.0, 1.0, 3.0]))
+    for left, right in ((a, b), (b, a)):
+        got = (bpd.DataFrame(left) + bpd.DataFrame(right))._to_pandas()
+        want = left + right
+        assert list(got.index) == list(want.index)
+        assert np.array_equal(got["c"].to_numpy(), want["c"].to_numpy(), equal_nan=True), (got, want)
+
+
 def test_binary_template_operand_shapes_are_bit_exact(cpu_device):
     """The Binary template's operand shapes -- scalars on either side, positional and labelled row vectors, a column
     Series along axis 0, co-partitioned frames, fused x*s+t chains -- on plain, wide (two column partitions), filtered
