@@ -24,6 +24,7 @@ ABI_VERSION = 3
 
 # enums (keep in sync with include/modin_b200.h)
 F64, I64, U8 = 0, 1, 2
+MAX_COLS = 32  # MB200_MAX_COLS: columns of one dtype per launch / value columns per group table
 
 OP = {
     "abs": 0, "neg": 1, "isna": 2, "notna": 3, "fillna_s": 4, "affine": 5,

@@ -47,10 +47,14 @@ struct mb200_join_table {
   int* rows;
   int persisted;  // holds a reference on the persisting L2 carve-out
   size_t carve_bytes, window_bytes;
-  // key-ordered copies of float64 payload columns (dense tables; see join_order_payload_kernel)
-  int nordered;
-  const void* ordered_src[MB200_MAX_COLS];
-  double* ordered[MB200_MAX_COLS];
+  // key-ordered copies of float64 payload columns (dense tables; see join_order_payload_kernel), one per source
+  // column and kept until the table is destroyed: a payload wider than one launch is probed in several launches,
+  // each of which finds its own columns' copies (malloc'd arrays of ordered_cap entries).  Nothing is evicted: every
+  // distinct source column costs range * 8 bytes of device memory until the table is destroyed.  A merge's table lives
+  // with its dim frame and is probed with that frame's payload columns only, so this is one copy per dim column.
+  int nordered, ordered_cap;
+  const void** ordered_src;
+  double** ordered;
 };
 
 namespace mb200 {
@@ -497,6 +501,8 @@ extern "C" int mb200_join_destroy(mb200_join_table* t, mb200_stream_t stream) {
   if (t->rows) cudaFreeAsync(t->rows, (cudaStream_t)stream);
   for (int c = 0; c < t->nordered; ++c)
     if (t->ordered[c]) cudaFreeAsync(t->ordered[c], (cudaStream_t)stream);
+  free(t->ordered_src);
+  free(t->ordered);
   if (t->meta) cudaFreeAsync(t->meta, (cudaStream_t)stream);
   if (t->persisted) l2_carveout_release();
   delete t;
@@ -575,6 +581,35 @@ extern "C" int mb200_join_probe(mb200_join_table* t, const int64_t* fact_keys, i
   return 0;
 }
 
+// The key-ordered copy of one float64 payload column of a dense table: found by source pointer, or built and kept.
+static int ordered_payload(mb200_join_table* t, const void* src, cudaStream_t st, const double** out) {
+  for (int i = 0; i < t->nordered; ++i)
+    if (t->ordered_src[i] == src) {
+      *out = t->ordered[i];
+      return 0;
+    }
+  if (t->nordered == t->ordered_cap) {
+    const int cap = t->ordered_cap ? 2 * t->ordered_cap : MB200_MAX_COLS;
+    const void** s = static_cast<const void**>(realloc(t->ordered_src, cap * sizeof(*s)));
+    if (!s) return fail("mb200_join_probe_gather", "out of host memory");
+    t->ordered_src = s;
+    double** o = static_cast<double**>(realloc(t->ordered, cap * sizeof(*o)));
+    if (!o) return fail("mb200_join_probe_gather", "out of host memory");
+    t->ordered = o;
+    t->ordered_cap = cap;
+  }
+  int grid;
+  if (int rc = launch_grid((long long)t->range, 256, 8, &grid)) return rc;
+  double* ord = nullptr;
+  MB_CUDA(cudaMallocAsync((void**)&ord, (size_t)t->range * 8, st));
+  t->ordered_src[t->nordered] = src;
+  t->ordered[t->nordered++] = ord;
+  join_order_payload_kernel<<<grid, 256, 0, st>>>(t->rows, t->range, static_cast<const double*>(src), ord);
+  MB_LAUNCH_CHECK("join_order_payload_kernel");
+  *out = ord;
+  return 0;
+}
+
 extern "C" int mb200_join_probe_gather(mb200_join_table* t, const int64_t* fact_keys, int64_t nfact, int ncols,
                                        const void* const* dim_cols, int dim_dtype, void* const* out_cols,
                                        int64_t* out_nmatch_dev, mb200_stream_t stream) {
@@ -603,29 +638,11 @@ extern "C" int mb200_join_probe_gather(mb200_join_table* t, const int64_t* fact_
     // (MB200_JOIN_ORDERED=0 keeps the two-read probe)
     const char* oe = getenv("MB200_JOIN_ORDERED");
     if (!(oe && oe[0] == '0')) {
-      bool same = t->nordered == ncols;
-      for (int c = 0; same && c < ncols; ++c) same = t->ordered_src[c] == dim_cols[c];
-      if (!same) {
-        for (int c = 0; c < t->nordered; ++c)
-          if (t->ordered[c]) cudaFreeAsync(t->ordered[c], st);
-        t->nordered = 0;
-        int ogrid;
-        if (int rc = launch_grid((long long)t->range, 256, 8, &ogrid)) return rc;
-        for (int c = 0; c < ncols; ++c) {
-          t->ordered[c] = nullptr;
-          MB_CUDA(cudaMallocAsync((void**)&t->ordered[c], (size_t)t->range * 8, st));
-          t->ordered_src[c] = dim_cols[c];
-          t->nordered = c + 1;
-          join_order_payload_kernel<<<ogrid, 256, 0, st>>>(t->rows, t->range, static_cast<const double*>(dim_cols[c]),
-                                                          t->ordered[c]);
-          MB_LAUNCH_CHECK("join_order_payload_kernel");
-        }
-      }
       OrderedParams op;
       memset(&op, 0, sizeof(op));
       op.ncols = ncols;
       for (int c = 0; c < ncols; ++c) {
-        op.ord[c] = t->ordered[c];
+        if (int rc = ordered_payload(t, dim_cols[c], st, &op.ord[c])) return rc;
         op.out[c] = static_cast<double*>(out_cols[c]);
       }
       join_dense_ordered_probe_kernel<<<grid, 256, 0, st>>>(t->kmin, t->range, fk, nfact, op);

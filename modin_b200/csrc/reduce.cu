@@ -78,13 +78,16 @@ struct Acc<MB200_RED_SUM, double> {
 };
 // Sum of squared deviations from a per-column centre: the second pass of pandas' two-pass variance
 // (nanops.nanvar: avg = sum / count; sqr = (avg - values) ** 2; NaNs dropped; result = sqr.sum() / (count - ddof)).
-// One rounding for the difference, one for the square, compensated summation like SUM.
+// One rounding for the difference, one for the square, compensated summation like SUM.  skipna drops the rows whose
+// VALUE is NaN, not the deviations that are: a column holding inf has centre inf and inf - inf = NaN, and pandas'
+// variance of it is NaN.
 template <>
 struct Acc<MB200_RED_SSD, double> : Acc<MB200_RED_SUM, double> {
   double center = 0.0;
   __device__ __forceinline__ void add(double x, int skipna) {
     const double d = __dsub_rn(center, x);
-    Acc<MB200_RED_SUM, double>::add(__dmul_rn(d, d), skipna);
+    const bool nan = x != x;
+    Acc<MB200_RED_SUM, double>::add(nan ? x : __dmul_rn(d, d), nan ? skipna : 0);
   }
 };
 template <>

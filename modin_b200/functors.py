@@ -1424,6 +1424,9 @@ def _lib_max_cols() -> int:
 
 
 # ------------------------------------------------------------------ broadcast merge functor
+_BOOL_MISSES = "device merge(how='left') with a bool payload column and unmatched left rows (pandas gives object dtype)"
+
+
 class DevMerge(DevFn):
     """Per-row-partition ``pandas.merge(left_block, right, how, on / left_on / right_on, sort=False)`` of
     MergeImpl.row_axis_merge (merge.py:139-168) as a join-table probe + payload gather.
@@ -1513,14 +1516,25 @@ class DevMerge(DevFn):
         pay_pos, ll, rl = self.result_labels(left.columns, right.columns)
         pay_cols = [right.cols[i] for i in pay_pos]
         has_int = any(c.dtype == np.int64 for c in pay_cols)
+        # a left row without a match gets NaN in every payload column, which turns a bool column into pandas' object
+        # dtype: not on the device path.  Without misses, bool payload is gathered like any other column.
+        has_bool = self.how == "left" and any(c.dtype == np.bool_ for c in pay_cols)
         if not unique:
             lrows, rrows, misses = ops.expand_matches(fact_keys, right.column(self.right_on), keep_misses=self.how == "left")
+            if has_bool and misses:
+                raise NotImplementedError(_BOOL_MISSES)
             promote = self.how == "left" and has_int and (self.promote_ints if self.promote_ints is not None else misses > 0)
             pay = ops.cast_columns_f64(pay_cols) if promote else pay_cols
             cols = ops.take_columns(left.cols, lrows) + ops.take_columns(pay, rrows)
             return DeviceBlock(cols, pandas.Index(ll + rl), nrows=len(lrows), range_start=0)
         if self.how == "left":
             promote = self.promote_ints
+            if has_bool:
+                idx, nmatch = table.probe(fact_keys)
+                if promote or int(nmatch.item()) != left.nrows:
+                    raise NotImplementedError(_BOOL_MISSES)
+                return DeviceBlock(list(left.cols) + ops.take_columns(pay_cols, idx), pandas.Index(ll + rl),
+                                   nrows=left.nrows, range_start=left.range_start)  # fmt: skip
             if has_int and promote is None:
                 gathered, nmatch = table.probe_gather(fact_keys, pay_cols)
                 promote = int(nmatch.item()) != left.nrows  # misses: pandas promotes int payload to float64 NaN

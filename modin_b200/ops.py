@@ -125,8 +125,8 @@ def map_columns(
             odt = np.dtype("int64")
         else:
             odt = in0[idxs[0]].dtype
-        for k in range(0, len(idxs), 32):
-            sel = idxs[k : k + 32]
+        for k in range(0, len(idxs), _lib.MAX_COLS):
+            sel = idxs[k : k + _lib.MAX_COLS]
             outs = [DeviceColumn.empty(n, odt) for _ in sel]
             a = _lib.ptr_array([in0[j].ptr for j in sel])
             b = _lib.ptr_array([in1[j].ptr for j in sel]) if in1 is not None else None
@@ -457,8 +457,18 @@ def hash_aggregate(key_cols_vals, flags: int, capacity_hint: int, partial: bool 
     overflows.  Returns (keys, sums, cnts, sizes) device columns."""
     from .config import GroupbyDenseKeys
 
-    cap = max(int(capacity_hint), 1024)
     nvals = len(key_cols_vals[0][1]) if key_cols_vals[0][1] else 0
+    if nvals > _lib.MAX_COLS:
+        # a table holds at most MAX_COLS value columns: aggregate them MAX_COLS at a time.  Every pass sees the same
+        # keys, so every table holds the same groups; emitted in ascending key order, their rows line up.
+        parts = []
+        for k in range(0, nvals, _lib.MAX_COLS):
+            cut = lambda cols: cols[k : k + _lib.MAX_COLS] if cols else cols  # noqa: E731
+            items = [(it[0], cut(it[1])) + ((cut(it[2]),) + tuple(it[3:]) if len(it) > 2 else ()) for it in key_cols_vals]
+            parts.append(hash_aggregate(items, flags, capacity_hint, partial=partial, sort=True))
+        join = lambda cols: [c for cs in cols for c in cs] if cols[0] is not None else None  # noqa: E731
+        return parts[0][0], join([p[1] for p in parts]), join([p[2] for p in parts]), parts[0][3]
+    cap = max(int(capacity_hint), 1024)
     total_rows = sum(len(item[0]) for item in key_cols_vals)
     skewed = False
     if total_rows > 0:
@@ -535,25 +545,31 @@ class JoinTable:
         for j, c in enumerate(dim_cols):
             groups.setdefault(c.code, []).append(j)
         # the match count is only needed to decide whether int64 payload has to be promoted (misses -> NaN), so
-        # only the int64 launch counts; float64-only payload lets the library probe its key-ordered payload
-        # copies (one random read per row).  The table caches those copies by source pointer: keep the
-        # source columns alive as long as the table is.
-        count_code = _lib.I64 if _lib.I64 in groups else None
-        self._payload_refs = list(dim_cols)
+        # only the first int64 launch counts; float64-only payload lets the library probe its key-ordered payload
+        # copies (one random read per row).  The table caches those copies per source column, by pointer: keep
+        # every source column alive as long as the table is.  Neither side evicts: a table is meant to be probed with
+        # the payload columns of its own dim frame.
+        if any(code == _lib.U8 for code in groups):
+            raise TypeError("bool payload columns are not on the device merge path")
+        counted = _lib.I64 not in groups
+        refs = self.__dict__.setdefault("_payload_refs", {})
         for code, idxs in groups.items():
-            if code == _lib.U8:
-                raise TypeError("bool payload columns are not on the device merge path")
-            sel_out = [DeviceColumn.empty(n, dim_cols[j].dtype) for j in idxs]
-            with _timed("join_probe_gather"):
-                _lib.check(
-                    self.lib.mb200_join_probe_gather(
-                        self.handle, fact_keys.ptr, n, len(idxs), _lib.ptr_array([dim_cols[j].ptr for j in idxs]), code,
-                        _lib.ptr_array([c.ptr for c in sel_out]), nm.data_ptr() if code == count_code else None,
-                        current_stream(),
-                    )
-                )  # fmt: skip
-            for j, c in zip(idxs, sel_out):
-                outs[j] = c
+            for k in range(0, len(idxs), _lib.MAX_COLS):
+                sel = idxs[k : k + _lib.MAX_COLS]
+                refs.update((dim_cols[j].ptr, dim_cols[j]) for j in sel)
+                sel_out = [DeviceColumn.empty(n, dim_cols[j].dtype) for j in sel]
+                count = not counted and code == _lib.I64
+                counted = counted or count
+                with _timed("join_probe_gather"):
+                    _lib.check(
+                        self.lib.mb200_join_probe_gather(
+                            self.handle, fact_keys.ptr, n, len(sel), _lib.ptr_array([dim_cols[j].ptr for j in sel]),
+                            code, _lib.ptr_array([c.ptr for c in sel_out]), nm.data_ptr() if count else None,
+                            current_stream(),
+                        )
+                    )  # fmt: skip
+                for j, c in zip(sel, sel_out):
+                    outs[j] = c
         return outs, nm
 
     def close(self):
@@ -611,8 +627,8 @@ def take_columns(cols: Sequence[DeviceColumn], idx: DeviceColumn) -> List[Device
     for j, c in enumerate(cols):
         groups.setdefault(c.code, []).append(j)
     for code, idxs in groups.items():
-        for k in range(0, len(idxs), 32):
-            sel = idxs[k : k + 32]
+        for k in range(0, len(idxs), _lib.MAX_COLS):
+            sel = idxs[k : k + _lib.MAX_COLS]
             o = [DeviceColumn.empty(n, cols[j].dtype) for j in sel]
             _lib.check(lib.mb200_take(code, len(sel), _lib.ptr_array([cols[j].ptr for j in sel]), idx.ptr, n,
                                       _lib.ptr_array([c.ptr for c in o]), current_stream()))  # fmt: skip

@@ -430,7 +430,7 @@ def cum_apply(state, cols, carries=None):
                     r = pandas.Series(x).ffill().to_numpy()
                     r = np.where(np.isnan(r), carry, r)
                 else:
-                    v = np.where(nan, 0.0 if op == "sum" else ident, x)
+                    v = np.where(nan, x.dtype.type(0) if op == "sum" else ident, x)  # int64 stays int64 (and wraps)
                     acc = {"sum": np.cumsum, "max": np.maximum.accumulate, "min": np.minimum.accumulate}[op](v)
                     r = _cum_comb(op, np.full(len(x), carry, dtype=x.dtype), acc).astype(x.dtype)
                     if x.dtype == np.float64:
