@@ -1,23 +1,28 @@
-"""Several int64 group keys as ONE: the order-preserving packing behind ``df.groupby([k1, k2, ...])``.
+"""Group keys of a device groupby, for both front doors: how the keys become the ONE int64 key column the single-key
+device groupby runs on (``key_image``), how the result's keys are restored (``restore_keys``), and how a dictionary
+aggregation is split per function and zipped back (``split_aggregations`` / ``zip_aggregations``).  Everything here
+works on lists of device blocks, one per row partition; each front door wraps them into its own frame type.
 
-The reference hands ``df.groupby([...])`` to pandas per block (alg/groupby.py:124-208), which builds a combined group
-index with ``get_group_index``.  Here the key tuples are packed into one int64 on the device,
-``sum_i (k_i - min_i) * stride_i`` with ``stride_i = prod_{j>i} (max_j - min_j + 1)``, the single-key device groupby
-(dense or hashed table) runs on the image, and the G result keys are unpacked afterwards -- per row one subtract +
-multiply per key column and k - 1 adds; per GROUP one divmod on the host (result-sized, not row-sized).  The key
-ranges come from the columns' cached statistics (``ops.key_stats``), agreed across ranks once.
+Several int64 keys are packed.  The reference hands ``df.groupby([...])`` to pandas per block (alg/groupby.py:124-208),
+which builds a combined group index with ``get_group_index``.  Here the key tuples are packed into one int64 on the
+device, ``sum_i (k_i - min_i) * stride_i`` with ``stride_i = prod_{j>i} (max_j - min_j + 1)``, the single-key device
+groupby (dense or hashed table) runs on the image, and the G result keys are unpacked afterwards -- per row one
+subtract + multiply per key column and k - 1 adds; per GROUP one divmod on the host (result-sized, not row-sized).  The
+key ranges come from the columns' cached statistics (``ops.key_stats``), agreed across ranks once.
 """
 
 from __future__ import annotations
 
-from typing import List, Sequence
+from typing import Dict, List, Sequence
 
 import numpy as np
+import pandas
 
 from . import dist, ops
 from .block import DeviceBlock, DeviceColumn
 
 PACKED_KEY = "__packed_key__"
+FLOAT_KEY = "float64 image"  # the restore description of one float64 key (``key_image``)
 
 
 def packing_plan(key_blocks: Sequence[DeviceBlock]):
@@ -98,4 +103,84 @@ def float_keys(image: DeviceColumn) -> np.ndarray:
     keys = bits.view(np.float64).copy()
     keys[img == _I64_MAX] = np.nan
     return keys
+
+
+# ---- the key image and the restore -------------------------------------------------------------------------------
+def key_image(key_blocks: List[DeviceBlock]):
+    """(image blocks, restore description) for the key columns of a groupby, one block per row partition.
+
+    One int64 key: the blocks themselves and ``None`` -- nothing is launched or allocated.  One float64 key: its
+    order-preserving image under the key's own label (``float_image``) and ``FLOAT_KEY``.  Several int64 keys: their
+    packed image labelled ``PACKED_KEY`` and ``(packing plan, key labels)``."""
+    first = key_blocks[0]
+    if len(first.cols) > 1:
+        plan = packing_plan(key_blocks)
+        label = pandas.Index([PACKED_KEY])
+        images = [DeviceBlock([pack(b, plan)], label, nrows=b.nrows, range_start=b.range_start) for b in key_blocks]
+        return images, (plan, list(first.columns))
+    if first.cols[0].dtype == np.float64:
+        return [DeviceBlock([float_image(b.cols[0])], b.columns, nrows=b.nrows, range_start=b.range_start)
+                for b in key_blocks], FLOAT_KEY  # fmt: skip
+    return key_blocks, None
+
+
+def restore_keys(blocks: List[DeviceBlock], image, dropna: bool = True, names=None) -> List[DeviceBlock]:
+    """Result blocks of a groupby on ``key_image``'s image, with the original keys as index columns: unpacked
+    several keys, or the float64 keys -- whose NaN group (the last row, if any) is dropped under ``dropna``.  ``names``
+    replaces the index names (``groupby(level=)``: the level's name)."""
+    out = []
+    for b in blocks:
+        keys, key_names = b.index_cols, b.index_names
+        if image == FLOAT_KEY:
+            host = float_keys(keys[0]) if b.nrows else np.zeros(0, dtype=np.float64)
+            if dropna and b.nrows and np.isnan(host[-1]):
+                b, host = b.slice_rows(0, b.nrows - 1), host[:-1]
+            keys = [DeviceColumn.from_numpy(host)]
+        elif image is not None:
+            plan, key_names = image
+            keys = unpack(keys[0], plan)
+        nb = DeviceBlock(b.cols, b.columns, nrows=b.nrows, index_cols=keys, index_names=names or key_names)
+        nb.keys_sorted_unique = True
+        out.append(nb)
+    return out
+
+
+# ---- dictionary aggregation --------------------------------------------------------------------------------------
+_DICT_AGGS = ("sum", "count", "mean", "min", "max")
+
+
+def split_aggregations(spec: dict, columns, keys=()) -> Dict[str, list]:
+    """``{column: function}`` -> ``{function: [columns]}``, in first-seen order.  ``groupby.agg`` with a dictionary
+    runs one device aggregation per DISTINCT function over the columns that ask for it (the reference's
+    ``_groupby_dict_reduce``, qc.py:3876-3970, builds one map / reduce table per function the same way)."""
+    by_func = {}
+    for col, fn in spec.items():
+        if not isinstance(fn, str) or fn not in _DICT_AGGS:
+            raise NotImplementedError(f"groupby.agg({{{col!r}: {fn!r}}}) is not on the B200 path")
+        if col not in columns or col in keys:
+            raise KeyError(col)
+        by_func.setdefault(fn, []).append(col)
+    return by_func
+
+
+def zip_aggregations(spec: dict, by_func: Dict[str, list], results: List[List[list]]) -> List[DeviceBlock]:
+    """One block per row partition holding ``spec``'s columns in its order, taken from the per-function results
+    (``results[i]``: the rows of ``by_func``'s i-th aggregation, each row the list of its column partitions' blocks).
+    Every result carries the same ascending group keys, so the columns are zipped as they are: buffers shared."""
+    where = {c: (i, j) for i, cols in enumerate(by_func.values()) for j, c in enumerate(cols)}
+    if any(len(row) != 1 for rows in results for row in rows):
+        raise NotImplementedError("dictionary aggregation over more than 32 columns per function")
+    if len({len(rows) for rows in results}) != 1:
+        raise NotImplementedError("per-function results are partitioned differently")
+    out = []
+    for row in zip(*results):
+        blks = [r[0] for r in row]
+        if len({b.nrows for b in blks}) != 1:
+            raise NotImplementedError("per-function results are partitioned differently")
+        nb = DeviceBlock([blks[i].cols[j] for i, j in (where[c] for c in spec)], pandas.Index(list(spec)),
+                         nrows=blks[0].nrows, index_cols=blks[0].index_cols, index_names=blks[0].index_names)  # fmt: skip
+        nb.keys_sorted_unique = True
+        nb.replicated = blks[0].replicated
+        out.append(nb)
+    return out
 

@@ -102,8 +102,9 @@ def register(shims: bool | None = None):
 
     from . import dist as bdist
     from . import functors as fx
+    from . import groupkeys as gk
     from . import partitioning as bp
-    from .block import DeviceBlock, DeviceColumn
+    from .block import DeviceBlock, concat_cols
     from .query_compiler import _dtypes_sum
 
     # ---------------------------------------------------------------- partition manager
@@ -202,7 +203,6 @@ def register(shims: bool | None = None):
         def __dataframe__(self, nan_as_null: bool = False, allow_copy: bool = True):
             """df.py:4803-4824, over the device blocks (``modin_b200.interchange``): buffers stay in HBM and say so
             (``__dlpack_device__`` = CUDA), one chunk per row partition."""
-            from .block import concat_cols
             from .interchange import B200ProtocolDataframe
 
             self._propagate_index_objs(axis=None)
@@ -373,73 +373,26 @@ def register(shims: bool | None = None):
                 if axis != 0 or not isinstance(by, type(query_compiler)) or len(by.columns) < 1:
                     raise NotImplementedError("device groupby: key columns of the same frame, axis=0")
                 frame, by_frame = query_compiler._modin_frame, by._modin_frame
-                plan = names = None
-                float_key = len(by.columns) == 1 and by_frame.has_materialized_dtypes and by.dtypes.iloc[0] == np.float64
-                if float_key:
-                    # a float64 key: the single-key groupby runs on its order-preserving int64 image (NaN = one group
-                    # that sorts last), the G result keys are mapped back afterwards (groupkeys.float_image / float_keys)
-                    from . import groupkeys as gk
-
-                    if by_frame._partitions.shape[1] != 1:
-                        raise NotImplementedError("device groupby: one key column partition")
+                # a float64 key or several int64 keys: the single-key groupby runs on their int64 image and the G
+                # result keys are restored afterwards (groupkeys.py); one int64 key is its own image
+                keys = [concat_cols([p.get() for p in row]) if len(row) > 1 else row[0].get() for row in by_frame._partitions]
+                images, image = gk.key_image(keys)
+                if image is not None:
                     pc = by_frame._partition_mgr_cls._partition_class
-                    rows = [row[0].get() for row in by_frame._partitions]
-                    parts = np.array([[pc(DeviceBlock([gk.float_image(b.cols[0])], b.columns, nrows=b.nrows,
-                                                      range_start=b.range_start))] for b in rows], dtype=object)  # fmt: skip
-                    by_frame = type(by_frame)(parts, by_frame.copy_index_cache(), by_frame.copy_columns_cache(),
-                                              by_frame.row_lengths, [1])  # fmt: skip
-                if len(by.columns) > 1:
-                    # several int64 keys: packed into one order-preserving int64 on the device (groupkeys.py), the
-                    # single-key groupby runs on the image, the G result keys are unpacked into index columns
-                    from . import groupkeys as gk
-                    from .block import concat_cols
-
-                    names = list(by.columns)
-                    if drop:
-                        keep = [c for c in query_compiler.columns if c not in set(names)]
-                        frame = query_compiler.getitem_column_array(keep)._modin_frame
-                    rows = [concat_cols([p.get() for p in row]) if len(row) > 1 else row[0].get() for row in by_frame._partitions]
-                    plan = gk.packing_plan(rows)
-                    pc = by_frame._partition_mgr_cls._partition_class
-                    label = pandas.Index([gk.PACKED_KEY])
-                    parts = np.array([[pc(DeviceBlock([gk.pack(b, plan)], label, nrows=b.nrows, range_start=b.range_start))]
-                                      for b in rows], dtype=object)  # fmt: skip
-                    by_frame = type(by_frame)(parts, by_frame.copy_index_cache(), label, by_frame.row_lengths, [1])
+                    by_frame = type(by_frame)(np.array([[pc(b)] for b in images], dtype=object), by_frame.copy_index_cache(),
+                                              images[0].columns, by_frame.row_lengths, [1])  # fmt: skip
+                if drop and len(by.columns) > 1:  # the packed key has a label of its own: the key columns leave here
+                    keep = [c for c in query_compiler.columns if c not in set(by.columns)]
+                    frame = query_compiler.getitem_column_array(keep)._modin_frame
                 # the functors themselves, not lambdas around them: the partition manager recognises them and fuses
                 # map + reduce into one direct-addressed table per GPU when the key range allows (pm.groupby_reduce)
                 new_frame = frame.groupby_reduce(axis, by_frame, map_f, red_f)
-                if plan is not None:
+                if image is not None or level is not None:
+                    # the private key label of groupby(level=) gives way to the index level's own name
+                    blocks = gk.restore_keys([row[0].get() for row in new_frame._partitions], image,
+                                             groupby_kwargs.get("dropna", True), [level_name] if level is not None else None)
                     pc = new_frame._partition_mgr_cls._partition_class
-                    rows = []
-                    for row in new_frame._partitions:
-                        b = row[0].get()
-                        nb = DeviceBlock(b.cols, b.columns, nrows=b.nrows, index_cols=gk.unpack(b.index_cols[0], plan),
-                                         index_names=names)  # fmt: skip
-                        nb.keys_sorted_unique = True
-                        rows.append([pc(nb)])
-                    new_frame = type(new_frame)(np.array(rows, dtype=object), None, None, None, None)
-                if level is not None and not float_key and plan is None:
-                    pc = new_frame._partition_mgr_cls._partition_class
-                    rows = []
-                    for row in new_frame._partitions:  # the private key label gives way to the index level's own name
-                        b = row[0].get()
-                        nb = DeviceBlock(b.cols, b.columns, nrows=b.nrows, index_cols=b.index_cols, index_names=[level_name])
-                        nb.keys_sorted_unique = True
-                        rows.append([pc(nb)])
-                    new_frame = type(new_frame)(np.array(rows, dtype=object), None, None, None, None)
-                if float_key:
-                    pc = new_frame._partition_mgr_cls._partition_class
-                    rows = []
-                    for row in new_frame._partitions:
-                        b = row[0].get()
-                        keys = gk.float_keys(b.index_cols[0]) if b.nrows else np.zeros(0, dtype=np.float64)
-                        if groupby_kwargs.get("dropna", True) and b.nrows and np.isnan(keys[-1]):
-                            b, keys = b.slice_rows(0, b.nrows - 1), keys[:-1]  # the NaN group is the last row, if any
-                        nb = DeviceBlock(b.cols, b.columns, nrows=b.nrows, index_cols=[DeviceColumn.from_numpy(keys)],
-                                         index_names=[level_name] if level is not None else b.index_names)  # fmt: skip
-                        nb.keys_sorted_unique = True
-                        rows.append([pc(nb)])
-                    new_frame = type(new_frame)(np.array(rows, dtype=object), None, None, None, None)
+                    new_frame = type(new_frame)(np.array([[pc(b)] for b in blocks], dtype=object), None, None, None, None)
                 if not groupby_kwargs.get("as_index", True):
                     from .query_compiler import group_keys_to_columns
 
@@ -569,43 +522,20 @@ def register(shims: bool | None = None):
                 raise NotImplementedError(f"groupby.agg({agg_func!r}) is not on the B200 path")
             if not isinstance(by, type(self)):
                 raise NotImplementedError("device groupby: key columns of the same frame, axis=0")
-            keys = set(by.columns) if drop else set()
-            by_func = {}
-            for col, fn in agg_func.items():
-                if isinstance(fn, (list, tuple)) and len(fn) == 1:
-                    fn = fn[0]
-                if not isinstance(fn, str) or fn not in self._DEVICE_AGGS or fn == "size":
-                    raise NotImplementedError(f"groupby.agg({{{col!r}: {fn!r}}}) is not on the B200 path")
-                if col not in self.columns or col in keys:
-                    raise KeyError(col)
-                by_func.setdefault(fn, []).append(col)
+            spec = {col: fn[0] if isinstance(fn, (list, tuple)) and len(fn) == 1 else fn for col, fn in agg_func.items()}
+            by_func = gk.split_aggregations(spec, self.columns, set(by.columns) if drop else ())
             if any(isinstance(fn, (list, tuple)) for fn in agg_func.values()):
                 raise NotImplementedError("groupby.agg with lists of functions (two-level result columns)")
             kw = dict(groupby_kwargs, as_index=True)
-            where, frames = {}, []
+            results = []
             for fn, cols in by_func.items():
                 res = getattr(self.getitem_column_array(cols), f"groupby_{fn}")(
                     by=by, axis=axis, groupby_kwargs=kw, agg_args=(), agg_kwargs={}, drop=False
                 )
-                frame = res._modin_frame
-                if frame._partitions.shape[1] != 1:
-                    raise NotImplementedError("dictionary aggregation over more than 32 columns per function")
-                for j, c in enumerate(cols):
-                    where[c] = (len(frames), j)
-                frames.append(frame)
-            if len({f._partitions.shape[0] for f in frames}) != 1:
-                raise NotImplementedError("per-function results are partitioned differently")
-            pc, rows = frames[0]._partition_mgr_cls._partition_class, []
-            for i in range(frames[0]._partitions.shape[0]):
-                blks = [f._partitions[i, 0].get() for f in frames]
-                if len({b.nrows for b in blks}) != 1:
-                    raise NotImplementedError("per-function results are partitioned differently")
-                nb = DeviceBlock([blks[where[c][0]].cols[where[c][1]] for c in agg_func], pandas.Index(list(agg_func)),
-                                 nrows=blks[0].nrows, index_cols=blks[0].index_cols, index_names=blks[0].index_names)  # fmt: skip
-                nb.keys_sorted_unique = True
-                nb.replicated = getattr(blks[0], "replicated", False)
-                rows.append([pc(nb)])
-            new_frame = type(frames[0])(np.array(rows, dtype=object), None, None, None, None)
+                results.append([[p.get() for p in row] for row in res._modin_frame._partitions])
+            pc = self._modin_frame._partition_mgr_cls._partition_class
+            rows = [[pc(b)] for b in gk.zip_aggregations(spec, by_func, results)]
+            new_frame = type(self._modin_frame)(np.array(rows, dtype=object), None, None, None, None)
             if not groupby_kwargs.get("as_index", True):
                 from .query_compiler import group_keys_to_columns
 

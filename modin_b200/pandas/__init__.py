@@ -18,8 +18,10 @@ from typing import Optional
 import numpy as np
 import pandas
 
+from .. import groupkeys as gk
 from ..functors import MODIN_UNNAMED_SERIES_LABEL
-from ..query_compiler import B200QueryCompiler
+from ..dataframe import B200Dataframe
+from ..query_compiler import B200QueryCompiler, group_keys_to_columns
 
 
 def _is_scalar(x):
@@ -383,10 +385,30 @@ class DataFrame(BasePandasDataset):
             raise NotImplementedError("groupby(axis=1) is not on the B200 path")
         if level is not None:
             raise NotImplementedError("groupby(level=) is not on the B200 path")
+        if as_index not in (True, False):  # the aggregations ask the template for as_index=True and apply it themselves
+            raise NotImplementedError(f"groupby(as_index={as_index!r}) is not on the B200 path")
         kwargs = dict(as_index=as_index, sort=sort, group_keys=group_keys, observed=observed, dropna=dropna, level=level)
+        if isinstance(by, (list, tuple)) and len(by) != 1:
+            # several int64 keys: the groupby runs on their packed image, which takes the key columns' place
+            from ..block import DeviceBlock, concat_cols
+
+            for k in by:
+                if k not in self.columns:
+                    raise KeyError(k)
+            if len(set(by)) != len(by):
+                raise ValueError("duplicate key columns")
+            frame = self._query_compiler._modin_frame
+            rows = [concat_cols([p.get() for p in row]) if len(row) > 1 else row[0].get() for row in frame._partitions]
+            pos = [int(self.columns.get_loc(k)) for k in by]
+            images, image = gk.key_image([b.select_columns(pos) for b in rows])
+            keep = [j for j in range(len(self.columns)) if j not in pos]
+            labels = pandas.Index([self.columns[j] for j in keep] + [gk.PACKED_KEY])
+            blocks = [DeviceBlock([b.cols[j] for j in keep] + img.cols, labels, nrows=b.nrows, range_start=b.range_start)
+                      for b, img in zip(rows, images)]  # fmt: skip
+            packed = DataFrame(query_compiler=type(self._query_compiler)(B200Dataframe.from_blocks(blocks)))
+            return DataFrameGroupBy(packed, packed[gk.PACKED_KEY]._query_compiler, drop=True, groupby_kwargs=kwargs,
+                                    image=image)  # fmt: skip
         if isinstance(by, (list, tuple)):
-            if len(by) != 1:
-                return _multi_key_groupby(self, list(by), kwargs)
             by = by[0]
         drop = False
         if isinstance(by, Series):
@@ -538,113 +560,29 @@ class Series(BasePandasDataset):
         return Series(query_compiler=frame._query_compiler)
 
 
-_PACKED_KEY = "__packed_key__"
-
-
-def _multi_key_groupby(df: "DataFrame", by: list, groupby_kwargs: dict) -> "DataFrameGroupBy":
-    """``df.groupby([k1, k2, ...])`` over int64 key columns: the keys are PACKED into one int64,
-    ``sum_i (k_i - min_i) * stride_i`` with ``stride_i = prod_{j>i} (max_j - min_j + 1)`` -- an order-preserving image of
-    the key tuples -- and the single-key device groupby (dense or hashed table) runs on it; the G result keys are
-    unpacked into a MultiIndex afterwards.  The reference gets the same result from pandas' own
-    ``get_group_index`` inside ``df.groupby([...])`` per block (alg/groupby.py:124-208).
-
-    Per row: one int64 AFFINE sweep per key column and k - 1 adds (device); per GROUP: one divmod on the host
-    (result-sized, not row-sized)."""
-    from .. import dist, ops
-    from ..block import DeviceBlock, concat_cols
-    from ..dataframe import B200Dataframe
-
-    for k in by:
-        if k not in df.columns:
-            raise KeyError(k)
-    if len(set(by)) != len(by):
-        raise ValueError("duplicate key columns")
-    frame = df._query_compiler._modin_frame
-    rows = [concat_cols([p.get() for p in row]) if len(row) > 1 else row[0].get() for row in frame._partitions]
-    pos = [int(df.columns.get_loc(k)) for k in by]
-    for b in rows:
-        for p in pos:
-            if b.cols[p].dtype != np.int64:
-                raise NotImplementedError("multi-column groupby on the B200 path needs int64 key columns")
-    # global [min, max] of every key column (one all_gather across ranks so that every rank packs alike)
-    mins, maxs = [], []
-    for p in pos:
-        lo, hi = ops.key_stats([b.cols[p] for b in rows])[:2]  # column metadata (cached after the first query)
-        if dist.is_distributed():
-            import torch
-
-            per_rank = dist.all_gather_small(torch.tensor([lo, hi], dtype=torch.int64, device=ops.current_device()))
-            lo, hi = min(r[0] for r in per_rank), max(r[1] for r in per_rank)
-        if lo > hi:
-            lo = hi = 0  # no rows anywhere
-        mins.append(lo)
-        maxs.append(hi)
-    ranges = [hi - lo + 1 for lo, hi in zip(mins, maxs)]
-    strides = [1] * len(by)
-    for i in range(len(by) - 2, -1, -1):
-        strides[i] = strides[i + 1] * ranges[i + 1]
-    if strides[0] * ranges[0] >= 1 << 62:
-        raise NotImplementedError("the key ranges of this multi-column groupby do not pack into 62 bits")
-    keep = [j for j in range(len(df.columns)) if j not in pos]
-    blocks = []
-    for b in rows:
-        packed = None
-        for p, lo, s in zip(pos, mins, strides):
-            # (key - lo) * stride, in that order: -lo * stride alone need not fit int64 (epoch-ns keys next to a
-            # second key), the difference always does
-            term = ops.map_columns("mul_s", ops.map_columns("sub_s", [b.cols[p]], s0=[lo]), s0=[s])[0] if b.nrows else b.cols[p]
-            packed = term if packed is None else ops.map_columns("add", [packed], [term])[0]
-        cols = [b.cols[j] for j in keep] + [packed]
-        labels = pandas.Index([df.columns[j] for j in keep] + [_PACKED_KEY])
-        blocks.append(DeviceBlock(cols, labels, nrows=b.nrows, range_start=b.range_start))
-    tmp = DataFrame(query_compiler=type(df._query_compiler)(B200Dataframe.from_blocks(blocks)))
-    g = DataFrameGroupBy(tmp, tmp[_PACKED_KEY]._query_compiler, drop=True, groupby_kwargs=groupby_kwargs)
-    g._unpack = (list(by), mins, ranges, strides)
-    return g
-
-
-def _unpack_group_keys(result_qc, unpack):
-    """Packed int64 group keys -> one device index column per original key (G values: host divmod)."""
-    from ..block import DeviceBlock, DeviceColumn
-    from ..dataframe import B200Dataframe
-
-    names, mins, ranges, strides = unpack
-    frame = result_qc._modin_frame
-    blocks = []
-    for row in frame._partitions:
-        if len(row) != 1:
-            raise NotImplementedError("multi-column groupby results wider than one column partition")
-        b = row[0].get()
-        packed = b.index_cols[0].to_numpy().astype(np.int64)
-        icols = [DeviceColumn.from_numpy(((packed // s) % r + lo).astype(np.int64)) for lo, r, s in zip(mins, ranges, strides)]
-        nb = DeviceBlock(b.cols, b.columns, nrows=b.nrows, index_cols=icols, index_names=list(names))
-        nb.keys_sorted_unique = True
-        blocks.append(nb)
-    return type(result_qc)(B200Dataframe.from_blocks(blocks))
-
-
 class DataFrameGroupBy:
     """modin/pandas/groupby.py (``_wrap_aggregation`` :1829-1886)."""
 
-    _unpack = None  # set by _multi_key_groupby: (key labels, mins, ranges, strides)
-
-    def __init__(self, df: DataFrame, by_qc, drop, groupby_kwargs):
+    def __init__(self, df: DataFrame, by_qc, drop, groupby_kwargs, image=None):
         self._df = df
         self._query_compiler = df._query_compiler
         self._by = by_qc
         self._drop = drop
         self._kwargs = groupby_kwargs
+        self._image = image  # how the keys behind ``by_qc`` are restored (``groupkeys.key_image``)
 
     def _wrap_aggregation(self, qc_method, numeric_only=False, agg_args=None, agg_kwargs=None):
-        qc = self._query_compiler
-        if self._drop:
-            # the key column lives in the frame: value columns are all the others (alg/groupby.py:186-199)
-            pass
-        result_qc = qc_method(qc, by=self._by, axis=0, groupby_kwargs=self._kwargs, agg_args=agg_args or [],
-                              agg_kwargs=agg_kwargs or {}, drop=self._drop)  # fmt: skip
-        if self._unpack is not None:
-            result_qc = _unpack_group_keys(result_qc, self._unpack)
-        return DataFrame(query_compiler=result_qc)
+        result_qc = qc_method(self._query_compiler, by=self._by, axis=0, groupby_kwargs=dict(self._kwargs, as_index=True),
+                              agg_args=agg_args or [], agg_kwargs=agg_kwargs or {}, drop=self._drop)  # fmt: skip
+        return self._finish(result_qc._modin_frame)
+
+    def _finish(self, frame):
+        """The result with the original keys restored, then -- ``as_index=False`` -- turned into leading columns."""
+        if self._image is not None:
+            frame = B200Dataframe.from_blocks(gk.restore_keys([row[0].get() for row in frame._partitions], self._image))
+        if not self._kwargs.get("as_index", True):
+            frame = group_keys_to_columns(frame)  # alg/groupby.py:278-294
+        return DataFrame(query_compiler=type(self._query_compiler)(frame))
 
     def sum(self, numeric_only=False, min_count=0):
         if min_count:
@@ -677,48 +615,17 @@ class DataFrameGroupBy:
     def _dict_agg(self, spec):
         """``groupby(key).agg({column: function})`` -- qc._groupby_dict_reduce (qc.py:3876-3970) splits a dictionary
         aggregation into per-function map / reduce tables.  Here: one device aggregation per distinct function over
-        the columns that ask for it; every result has the same ascending keys, so the result blocks are zipped
-        column-wise on the device (buffers shared, nothing copied) in the dictionary's order."""
-        from ..block import DeviceBlock
-        from ..dataframe import B200Dataframe
-
+        the columns that ask for it, zipped column-wise in the dictionary's order (``groupkeys.zip_aggregations``)."""
         if not self._drop:
             raise NotImplementedError("dictionary aggregation needs the key column inside the frame")
         key = self._by.columns[0]
-        by_func = {}
-        for col, fn in spec.items():
-            if not isinstance(fn, str) or fn not in ("sum", "count", "mean", "min", "max"):
-                raise NotImplementedError(f"groupby.agg({{{col!r}: {fn!r}}}) is not on the B200 path")
-            if col not in self._df.columns or col == key:
-                raise KeyError(col)
-            by_func.setdefault(fn, []).append(col)
-        where = {}
-        frames = []
+        by_func = gk.split_aggregations(spec, self._df.columns, (key,))
+        kw = dict(self._kwargs, as_index=True)
+        results = []
         for fn, cols in by_func.items():
-            res = getattr(self._df[[key] + cols].groupby(key, **{k: v for k, v in self._kwargs.items() if k != "level"}), fn)()
-            frame = res._query_compiler._modin_frame
-            if frame._partitions.shape[1] != 1:
-                raise NotImplementedError("dictionary aggregation over more than 32 columns per function")
-            for j, c in enumerate(cols):
-                where[c] = (len(frames), j)
-            frames.append(frame)
-        nparts = {f._partitions.shape[0] for f in frames}
-        if len(nparts) != 1:
-            raise NotImplementedError("per-function results are partitioned differently")
-        blocks = []
-        for i in range(nparts.pop()):
-            blks = [f._partitions[i, 0].get() for f in frames]
-            if len({b.nrows for b in blks}) != 1:
-                raise NotImplementedError("per-function results are partitioned differently")
-            cols = [blks[where[c][0]].cols[where[c][1]] for c in spec]
-            nb = DeviceBlock(cols, pandas.Index(list(spec)), nrows=blks[0].nrows, index_cols=blks[0].index_cols,
-                             index_names=blks[0].index_names)  # fmt: skip
-            nb.keys_sorted_unique = True
-            blocks.append(nb)
-        qc = type(self._query_compiler)(B200Dataframe.from_blocks(blocks))
-        if self._unpack is not None:
-            qc = _unpack_group_keys(qc, self._unpack)
-        return DataFrame(query_compiler=qc)
+            res = getattr(self._df[[key] + cols].groupby(key, **kw), fn)()
+            results.append([[p.get() for p in row] for row in res._query_compiler._modin_frame._partitions])
+        return self._finish(B200Dataframe.from_blocks(gk.zip_aggregations(spec, by_func, results)))
 
     aggregate = agg
 

@@ -194,6 +194,10 @@ def test_groupby_dictionary_aggregation(cpu_device, dense):
         want = pdf.groupby("key").agg(spec)
         assert list(got.columns) == list(want.columns) and list(got.index) == list(want.index) and got.index.name == "key"
         assert np.allclose(got.to_numpy(dtype=np.float64), want.to_numpy(dtype=np.float64), rtol=0, atol=1e-9, equal_nan=True)
+        got = bpd.DataFrame(pdf).groupby("key", as_index=False).agg(spec)._to_pandas()
+        want = pdf.groupby("key", as_index=False).agg(spec)
+        assert list(got.columns) == list(want.columns) and got.index.equals(want.index)
+        assert np.allclose(got.to_numpy(dtype=np.float64), want.to_numpy(dtype=np.float64), rtol=0, atol=1e-9, equal_nan=True)
         with pytest.raises(NotImplementedError):
             bpd.DataFrame(pdf).groupby("key").agg({"c0": "median"})
         with pytest.raises(KeyError):
@@ -349,6 +353,11 @@ def test_multi_key_groupby_packs_the_keys(cpu_device, dense):
         got = df.groupby(["key", "k2"]).agg({"c1": "max", "c0": "sum"})._to_pandas()
         want = pdf.groupby(["key", "k2"]).agg({"c1": "max", "c0": "sum"})
         assert got.index.equals(want.index) and np.allclose(got.to_numpy(), want.to_numpy(), atol=1e-9, equal_nan=True)
+        # as_index=False: the keys are unpacked first, then become the leading columns
+        got = df.groupby(["key", "k2"], as_index=False).sum()._to_pandas()
+        want = pdf.drop(columns="k3").groupby(["key", "k2"], as_index=False).sum()
+        assert list(got.columns) == list(want.columns) and got.index.equals(want.index)
+        assert np.allclose(got.to_numpy(dtype=np.float64), want.to_numpy(dtype=np.float64), rtol=0, atol=1e-9, equal_nan=True)
         with pytest.raises(KeyError):
             df.groupby(["key", "nope"])
         with pytest.raises(NotImplementedError):
