@@ -117,9 +117,11 @@ enum mb200_reduce_op {
   MB200_RED_MAX = 2,
   MB200_RED_COUNT = 3, /* out_cnt only */
   MB200_RED_PROD = 4,  /* out_val = product (NaN skipped iff skipna), out_cnt = #non-NaN */
-  MB200_RED_SSD = 5    /* out_val = sum of (centre - x)^2 (NaN skipped iff skipna), out_cnt = #non-NaN:
+  MB200_RED_SSD = 5,   /* out_val = sum of (centre - x)^2 (NaN skipped iff skipna), out_cnt = #non-NaN:
                           the second pass of pandas' two-pass var / std (nanops.nanvar), float64 only,
                           through mb200_reduce_columns_centered */
+  MB200_RED_ARGMIN = 6, /* out_val = min over non-NaN, out_pos = first row holding it, out_cnt = #non-NaN:  */
+  MB200_RED_ARGMAX = 7  /* through mb200_reduce_arg_columns only                                           */
 };
 
 /* ---- groupby aggregate selection (bit flags) ------------------------------ */
@@ -189,6 +191,14 @@ int mb200_reduce_columns_centered(int op, int dtype, int ncols, const void* cons
                                   int skipna, const double* centers_dev, void* out_val,
                                   int64_t* out_cnt, void* scratch, int variant,
                                   mb200_stream_t stream);
+/* MB200_RED_ARGMIN / MB200_RED_ARGMAX over float64 or int64 columns, one read of every element: out_val[c] = the
+ * extreme value (column dtype), out_pos[c] = the first row holding it (-1 when no value is valid; out_val is then the
+ * identity, +-inf or the int64 limit), out_cnt[c] = #non-NaN.  NaN is skipped; -0.0 and 0.0 tie; a tie goes to the
+ * smaller row, so the result does not depend on tiles or CTAs.  Scratch and variants as for mb200_reduce_columns.
+ * Replaces the per-column work of Reduce.register(pandas.DataFrame.idxmax / idxmin) qc.py:1101-1102. */
+int mb200_reduce_arg_columns(int op, int dtype, int ncols, const void* const* in, int64_t nrows,
+                             void* out_val, int64_t* out_pos, int64_t* out_cnt, void* scratch,
+                             int variant, mb200_stream_t stream);
 
 /* ======================= GroupByReduce ===================================== */
 typedef struct mb200_gb_table mb200_gb_table; /* opaque, device resident */

@@ -37,7 +37,7 @@ OP = {
     "fma3": 64,
 }  # fmt: skip
 PREDICATES = {"isna", "notna", "eq_s", "ne_s", "lt_s", "le_s", "gt_s", "ge_s", "eq", "ne", "lt", "le", "gt", "ge"}
-RED = {"sum": 0, "min": 1, "max": 2, "count": 3, "prod": 4, "ssd": 5}
+RED = {"sum": 0, "min": 1, "max": 2, "count": 3, "prod": 4, "ssd": 5, "argmin": 6, "argmax": 7}
 CUM = {"sum": 0, "max": 1, "min": 2, "ffill": 3}
 GB_SUM, GB_COUNT, GB_SIZE, GB_MIN, GB_MAX = 1, 2, 4, 8, 16
 
@@ -69,6 +69,7 @@ _SIGNATURES = {
     "mb200_reduce_columns": (C.c_int, [C.c_int, C.c_int, C.c_int, _vpp, _i64, C.c_int, _vp, _vp, _vp, C.c_int, _vp]),
     "mb200_reduce_columns_centered": (C.c_int, [C.c_int, C.c_int, C.c_int, _vpp, _i64, C.c_int, _vp, _vp, _vp, _vp,
                                                 C.c_int, _vp]),
+    "mb200_reduce_arg_columns": (C.c_int, [C.c_int, C.c_int, C.c_int, _vpp, _i64, _vp, _vp, _vp, _vp, C.c_int, _vp]),
     "mb200_gb_create": (C.c_int, [_vpp, _i64, C.c_int, C.c_int, _vp]),
     "mb200_key_range": (C.c_int, [_vp, _i64, _vp, C.c_int, _vp]),
     "mb200_gb_create_dense": (C.c_int, [_vpp, _i64, _i64, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]),

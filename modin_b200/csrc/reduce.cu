@@ -15,7 +15,9 @@
 // compensation is dropped while the running sum is not finite, so +-inf inputs and sums that
 // overflow to +-inf behave like pandas/numpy).
 // Stage 2 (reduce_finalize) combines the per-CTA partials in fixed order.
-// Algorithmic traffic: 8 B read per element; output ncols * 16 B.
+// ARGMIN / ARGMAX (idxmin / idxmax) run through the same two kernels with the row index of every element carried
+// next to its value (known from the tile base), plus a position per CTA partial and their own stage 2.
+// Algorithmic traffic: 8 B read per element; output ncols * 16 B (24 B with positions).
 #include <math.h>
 #include <type_traits>
 
@@ -41,7 +43,11 @@ struct RedParams {
   void* part_val;       // [ncols][gridDim.x]
   long long* part_cnt;  // [ncols][gridDim.x]
   const double* centers;  // SSD only: per-column centre (device array [ncols])
+  long long* part_pos;    // ARGMIN / ARGMAX only: [ncols][gridDim.x]
 };
+
+template <int OP>
+constexpr bool kArgOp = OP == MB200_RED_ARGMIN || OP == MB200_RED_ARGMAX;
 
 // ---------------------------------------------------------------- accumulators
 template <int OP, typename T>
@@ -217,9 +223,103 @@ struct Acc<MB200_RED_COUNT, long long> {
   static __device__ __forceinline__ long long combine(long long a, long long) { return a; }
 };
 
+// (best, pos, n): the extreme value, the first row holding it, the number of non-NaN values.  A candidate wins when it
+// is strictly better or equal at a smaller row, a rule that is associative and commutative, so the answer does not
+// depend on the order rows and partials are combined in.  NaN fails every comparison and is skipped; the sentinel
+// position INT64_MAX loses every tie, so a column of -inf (or INT64_MIN) still finds its first row for ARGMAX.
+template <bool MAX, typename T>
+__host__ __device__ constexpr T arg_identity() {
+  if constexpr (std::is_same<T, double>::value)
+    return MAX ? -(double)INFINITY : (double)INFINITY;
+  else
+    return MAX ? (long long)0x8000000000000000ULL : 0x7fffffffffffffffLL;
+}
+template <bool MAX, typename T>
+struct ArgAcc {
+  T best = arg_identity<MAX, T>();
+  long long pos = 0x7fffffffffffffffLL;
+  long long n = 0;
+  __device__ __forceinline__ void take(T x, long long i) {
+    const bool win = (MAX ? x > best : x < best) || (x == best && i < pos);
+    best = win ? x : best;
+    pos = win ? i : pos;
+  }
+  __device__ __forceinline__ void add_at(T x, long long i) {
+    n += (x == x);
+    take(x, i);
+  }
+  __device__ __forceinline__ void merge(const ArgAcc& o) {
+    take(o.best, o.pos);
+    n += o.n;
+  }
+};
+template <typename T>
+struct Acc<MB200_RED_ARGMIN, T> : ArgAcc<false, T> {};
+template <typename T>
+struct Acc<MB200_RED_ARGMAX, T> : ArgAcc<true, T> {};
+
+// element x at row i into an accumulator: the arg-reductions keep the row, the others only the value
+template <int OP, typename T>
+__device__ __forceinline__ void feed(Acc<OP, T>& a, T x, long long i, int skipna) {
+  if constexpr (kArgOp<OP>)
+    a.add_at(x, i);
+  else
+    a.add(x, skipna);
+}
+
 template <typename T>
 __device__ __forceinline__ T shfl_xor(T v, int m) {
   return __shfl_xor_sync(0xffffffffu, v, m);
+}
+
+template <int OP, typename T>
+__device__ __forceinline__ void shfl_merge(Acc<OP, T>& a, int m) {
+  Acc<OP, T> o;
+  o.best = shfl_xor(a.best, m);
+  o.pos = shfl_xor(a.pos, m);
+  o.n = shfl_xor(a.n, m);
+  a.merge(o);
+}
+
+// block_combine for the arg-reductions: (value, pos, count) through the same two-level tree; result in thread 0
+template <int OP, typename T>
+__device__ __forceinline__ void block_combine_arg(Acc<OP, T>& a) {
+  __shared__ T s_val[32];
+  __shared__ long long s_pos[32];
+  __shared__ long long s_cnt[32];
+#pragma unroll
+  for (int m = 16; m >= 1; m >>= 1) shfl_merge(a, m);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nw = (blockDim.x + 31) >> 5;
+  if (lane == 0) {
+    s_val[warp] = a.best;
+    s_pos[warp] = a.pos;
+    s_cnt[warp] = a.n;
+  }
+  __syncthreads();
+  if (warp == 0) {
+    Acc<OP, T> w;
+    if (lane < nw) {
+      w.best = s_val[lane];
+      w.pos = s_pos[lane];
+      w.n = s_cnt[lane];
+    }
+#pragma unroll
+    for (int m = 16; m >= 1; m >>= 1) shfl_merge(w, m);
+    a = w;
+  }
+}
+
+// end of a reduce kernel: block-wide combine of acc, thread 0 writes this CTA's partial
+template <int OP, typename T>
+__device__ __forceinline__ void finish_arg(const RedParams& p, Acc<OP, T>& acc) {
+  block_combine_arg<OP, T>(acc);
+  if (threadIdx.x == 0) {
+    const size_t idx = (size_t)blockIdx.y * gridDim.x + blockIdx.x;
+    static_cast<T*>(p.part_val)[idx] = acc.best;
+    p.part_pos[idx] = acc.pos;
+    p.part_cnt[idx] = acc.n;
+  }
 }
 
 // block-wide combine of (value, count); result valid in thread 0.  Fixed tree => deterministic.
@@ -277,6 +377,9 @@ __global__ void __launch_bounds__(kRThreads) reduce_ldg_kernel(const __grid_cons
 #pragma unroll
     for (int i = 0; i < 4; ++i) acc[i].center = c;
   }
+  // the arg-reductions keep (value, row, count) per accumulator: one accumulator instead of four keeps them within
+  // the registers of the MAX instantiation (same occupancy); they are compare-and-select bound, not add-latency bound
+  constexpr int k1 = kArgOp<OP> ? 0 : 1, k2 = kArgOp<OP> ? 0 : 2, k3 = kArgOp<OP> ? 0 : 3;
   for (long long t = blockIdx.x; t < ntiles; t += gridDim.x) {
     const long long base = t * kLdgTile;
     if (VEC && base + kLdgTile <= n) {
@@ -286,10 +389,11 @@ __global__ void __launch_bounds__(kRThreads) reduce_ldg_kernel(const __grid_cons
         for (int u = 0; u < kLdgUnroll; ++u) v[u] = ldg_stream_f64x4(a + base + (long long)(u * kRThreads + tid) * 4);
 #pragma unroll
         for (int u = 0; u < kLdgUnroll; ++u) {
-          acc[0].add(v[u].x, p.skipna);
-          acc[1].add(v[u].y, p.skipna);
-          acc[2].add(v[u].z, p.skipna);
-          acc[3].add(v[u].w, p.skipna);
+          const long long i = base + (long long)(u * kRThreads + tid) * 4;
+          feed<OP, T>(acc[0], v[u].x, i, p.skipna);
+          feed<OP, T>(acc[k1], v[u].y, i + 1, p.skipna);
+          feed<OP, T>(acc[k2], v[u].z, i + 2, p.skipna);
+          feed<OP, T>(acc[k3], v[u].w, i + 3, p.skipna);
         }
       } else {
         i64x4 v[kLdgUnroll];
@@ -297,24 +401,29 @@ __global__ void __launch_bounds__(kRThreads) reduce_ldg_kernel(const __grid_cons
         for (int u = 0; u < kLdgUnroll; ++u) v[u] = ldg_stream_i64x4(a + base + (long long)(u * kRThreads + tid) * 4);
 #pragma unroll
         for (int u = 0; u < kLdgUnroll; ++u) {
-          acc[0].add(v[u].x, p.skipna);
-          acc[1].add(v[u].y, p.skipna);
-          acc[2].add(v[u].z, p.skipna);
-          acc[3].add(v[u].w, p.skipna);
+          const long long i = base + (long long)(u * kRThreads + tid) * 4;
+          feed<OP, T>(acc[0], v[u].x, i, p.skipna);
+          feed<OP, T>(acc[k1], v[u].y, i + 1, p.skipna);
+          feed<OP, T>(acc[k2], v[u].z, i + 2, p.skipna);
+          feed<OP, T>(acc[k3], v[u].w, i + 3, p.skipna);
         }
       }
     } else {
       const long long end = (base + kLdgTile < n) ? base + kLdgTile : n;
-      for (long long i = base + tid; i < end; i += kRThreads) acc[0].add(a[i], p.skipna);
+      for (long long i = base + tid; i < end; i += kRThreads) feed<OP, T>(acc[0], a[i], i, p.skipna);
     }
   }
   acc[0].merge(acc[1]);
   acc[2].merge(acc[3]);
   acc[0].merge(acc[2]);
-  T val = acc[0].value();
-  long long cnt = acc[0].n;
-  block_combine<OP, T>(val, cnt);
-  write_partial<OP, T>(p, val, cnt);
+  if constexpr (kArgOp<OP>) {
+    finish_arg<OP, T>(p, acc[0]);
+  } else {
+    T val = acc[0].value();
+    long long cnt = acc[0].n;
+    block_combine<OP, T>(val, cnt);
+    write_partial<OP, T>(p, val, cnt);
+  }
 }
 
 // ---------------------------------------------------------------- variant 0: TMA-staged tiles
@@ -383,26 +492,26 @@ __global__ void __launch_bounds__(kTmaThreads) reduce_tma_kernel(const __grid_co
       mbar_wait(&full[s], (uint32_t)((k / kStages) & 1));
       const T* tile = tiles + (size_t)s * kTmaTileElems;
       const int ne = tile_elems(k);
+      const long long base = (first + k * gridDim.x) * kTmaTileElems;  // row of tile[0]
       if (ne == kTmaTileElems) {
 #pragma unroll
         for (int j = 0; j < kTmaTileElems / (2 * kRThreads); ++j) {
           const int e = (j * kRThreads + tid) * 2;
           if constexpr (std::is_same<T, double>::value) {
             const double2 v = *reinterpret_cast<const double2*>(tile + e);
-            acc[(2 * j) & 3].add(v.x, p.skipna);
-            acc[(2 * j + 1) & 3].add(v.y, p.skipna);
+            feed<OP, T>(acc[(2 * j) & 3], v.x, base + e, p.skipna);
+            feed<OP, T>(acc[(2 * j + 1) & 3], v.y, base + e + 1, p.skipna);
           } else {
             const longlong2 v = *reinterpret_cast<const longlong2*>(tile + e);
-            acc[(2 * j) & 3].add(v.x, p.skipna);
-            acc[(2 * j + 1) & 3].add(v.y, p.skipna);
+            feed<OP, T>(acc[(2 * j) & 3], v.x, base + e, p.skipna);
+            feed<OP, T>(acc[(2 * j + 1) & 3], v.y, base + e + 1, p.skipna);
           }
         }
       } else {
         const int ne_even = ne & ~1;
-        for (int e = tid; e < ne_even; e += kRThreads) acc[0].add(tile[e], p.skipna);
+        for (int e = tid; e < ne_even; e += kRThreads) feed<OP, T>(acc[0], tile[e], base + e, p.skipna);
         if ((ne & 1) && tid == 0) {  // odd tail element never went through the 16-byte bulk copy
-          const long long base = (first + k * gridDim.x) * kTmaTileElems;
-          acc[1].add(a[base + ne - 1], p.skipna);
+          feed<OP, T>(acc[1], a[base + ne - 1], base + ne - 1, p.skipna);
         }
       }
       __syncwarp();
@@ -412,10 +521,14 @@ __global__ void __launch_bounds__(kTmaThreads) reduce_tma_kernel(const __grid_co
   acc[0].merge(acc[1]);
   acc[2].merge(acc[3]);
   acc[0].merge(acc[2]);
-  T val = acc[0].value();
-  long long cnt = acc[0].n;
-  block_combine<OP, T>(val, cnt);
-  write_partial<OP, T>(p, val, cnt);
+  if constexpr (kArgOp<OP>) {
+    finish_arg<OP, T>(p, acc[0]);
+  } else {
+    T val = acc[0].value();
+    long long cnt = acc[0].n;
+    block_combine<OP, T>(val, cnt);
+    write_partial<OP, T>(p, val, cnt);
+  }
 }
 
 // ---------------------------------------------------------------- stage 2
@@ -459,9 +572,33 @@ __global__ void reduce_finalize_kernel(const void* part_val, const long long* pa
   }
 }
 
+// Stage 2 of ARGMIN / ARGMAX: the same per-column warp pass, carrying the position; -1 when no value is valid.
+template <int OP, typename T>
+__global__ void reduce_arg_finalize_kernel(const void* part_val, const long long* part_pos, const long long* part_cnt,
+                                           int nparts, void* out_val, long long* out_pos, long long* out_cnt) {
+  const int col = blockIdx.x;
+  const int lane = threadIdx.x;
+  const size_t off = (size_t)col * nparts;
+  Acc<OP, T> a;
+  for (int i = lane; i < nparts; i += 32) {
+    Acc<OP, T> o;
+    o.best = static_cast<const T*>(part_val)[off + i];
+    o.pos = part_pos[off + i];
+    o.n = part_cnt[off + i];
+    a.merge(o);
+  }
+#pragma unroll
+  for (int m = 16; m >= 1; m >>= 1) shfl_merge(a, m);
+  if (lane == 0) {
+    static_cast<T*>(out_val)[col] = a.best;
+    out_pos[col] = a.n > 0 ? a.pos : -1;
+    out_cnt[col] = a.n;
+  }
+}
+
 template <int OP, typename T>
 static int run_reduce(const RedParams& p0, int variant, void* out_val, long long* out_cnt, void* scratch,
-                      cudaStream_t st) {
+                      cudaStream_t st, long long* out_pos = nullptr) {
   DevProps dp;
   if (int rc = dev_props(&dp)) return rc;
   RedParams p = p0;
@@ -493,6 +630,8 @@ static int run_reduce(const RedParams& p0, int variant, void* out_val, long long
   p.part_val = scratch;
   p.part_cnt = reinterpret_cast<long long*>(static_cast<char*>(scratch) +
                                             (size_t)MB200_MAX_COLS * kMaxCtasPerCol * 8);
+  p.part_pos = reinterpret_cast<long long*>(static_cast<char*>(scratch) +
+                                            (size_t)MB200_MAX_COLS * kMaxCtasPerCol * 16);
   dim3 grid((unsigned)per_col, (unsigned)p.ncols);
   if (variant == 0) {
     reduce_tma_kernel<OP, T><<<grid, kTmaThreads, smem, st>>>(p);
@@ -504,9 +643,15 @@ static int run_reduce(const RedParams& p0, int variant, void* out_val, long long
       reduce_ldg_kernel<OP, T, false><<<grid, kRThreads, 0, st>>>(p);
     MB_LAUNCH_CHECK("reduce_ldg_kernel");
   }
-  reduce_finalize_kernel<OP, T><<<p.ncols, 32, 0, st>>>(p.part_val, p.part_cnt, (int)per_col, p.nrows, p.skipna,
-                                                        out_val, out_cnt);
-  MB_LAUNCH_CHECK("reduce_finalize_kernel");
+  if constexpr (kArgOp<OP>) {
+    reduce_arg_finalize_kernel<OP, T><<<p.ncols, 32, 0, st>>>(p.part_val, p.part_pos, p.part_cnt, (int)per_col,
+                                                              out_val, out_pos, out_cnt);
+    MB_LAUNCH_CHECK("reduce_arg_finalize_kernel");
+  } else {
+    reduce_finalize_kernel<OP, T><<<p.ncols, 32, 0, st>>>(p.part_val, p.part_cnt, (int)per_col, p.nrows, p.skipna,
+                                                          out_val, out_cnt);
+    MB_LAUNCH_CHECK("reduce_finalize_kernel");
+  }
   return 0;
 }
 
@@ -516,18 +661,30 @@ using namespace mb200;
 
 extern "C" size_t mb200_reduce_scratch_bytes(int ncols) {
   (void)ncols;
-  return (size_t)MB200_MAX_COLS * kMaxCtasPerCol * 16;
+  return (size_t)MB200_MAX_COLS * kMaxCtasPerCol * 24;  // per-CTA values, counts and (arg-reductions) positions
 }
 
 static int reduce_columns_impl(int op, int dtype, int ncols, const void* const* in, int64_t nrows, int skipna,
                                const double* centers_dev, void* out_val, int64_t* out_cnt, void* scratch, int variant,
-                               mb200_stream_t stream);
+                               mb200_stream_t stream, int64_t* out_pos = nullptr);
 
 extern "C" int mb200_reduce_columns(int op, int dtype, int ncols, const void* const* in, int64_t nrows,
                                     int skipna, void* out_val, int64_t* out_cnt, void* scratch, int variant,
                                     mb200_stream_t stream) {
   if (op == MB200_RED_SSD) return fail("mb200_reduce_columns", "MB200_RED_SSD needs mb200_reduce_columns_centered");
+  if (op == MB200_RED_ARGMIN || op == MB200_RED_ARGMAX)
+    return fail("mb200_reduce_columns", "MB200_RED_ARGMIN / ARGMAX need mb200_reduce_arg_columns");
   return reduce_columns_impl(op, dtype, ncols, in, nrows, skipna, nullptr, out_val, out_cnt, scratch, variant, stream);
+}
+
+extern "C" int mb200_reduce_arg_columns(int op, int dtype, int ncols, const void* const* in, int64_t nrows,
+                                        void* out_val, int64_t* out_pos, int64_t* out_cnt, void* scratch, int variant,
+                                        mb200_stream_t stream) {
+  if (op != MB200_RED_ARGMIN && op != MB200_RED_ARGMAX)
+    return fail("mb200_reduce_arg_columns", "op must be MB200_RED_ARGMIN or MB200_RED_ARGMAX");
+  if (ncols > 0 && (!out_val || !out_pos || !out_cnt)) return fail("mb200_reduce_arg_columns", "null output");
+  return reduce_columns_impl(op, dtype, ncols, in, nrows, 1, nullptr, out_val, out_cnt, scratch, variant, stream,
+                             out_pos);
 }
 
 extern "C" int mb200_reduce_columns_centered(int op, int dtype, int ncols, const void* const* in, int64_t nrows,
@@ -542,7 +699,7 @@ extern "C" int mb200_reduce_columns_centered(int op, int dtype, int ncols, const
 
 static int reduce_columns_impl(int op, int dtype, int ncols, const void* const* in, int64_t nrows, int skipna,
                                const double* centers_dev, void* out_val, int64_t* out_cnt, void* scratch, int variant,
-                               mb200_stream_t stream) {
+                               mb200_stream_t stream, int64_t* out_pos) {
   if (ncols < 0 || ncols > MB200_MAX_COLS) return fail("mb200_reduce_columns", "ncols out of range (0..32)");
   if (nrows < 0) return fail("mb200_reduce_columns", "negative nrows");
   if (ncols == 0) return 0;
@@ -559,7 +716,8 @@ static int reduce_columns_impl(int op, int dtype, int ncols, const void* const* 
   p.centers = centers_dev;
   cudaStream_t st = (cudaStream_t)stream;
   long long* oc = reinterpret_cast<long long*>(out_cnt);
-#define MB_RED(OPC, T) return run_reduce<OPC, T>(p, variant, out_val, oc, scratch, st);
+  long long* op_pos = reinterpret_cast<long long*>(out_pos);
+#define MB_RED(OPC, T) return run_reduce<OPC, T>(p, variant, out_val, oc, scratch, st, op_pos);
   if (dtype == MB200_F64) {
     switch (op) {
       case MB200_RED_SUM: MB_RED(MB200_RED_SUM, double)
@@ -568,6 +726,8 @@ static int reduce_columns_impl(int op, int dtype, int ncols, const void* const* 
       case MB200_RED_COUNT: MB_RED(MB200_RED_COUNT, double)
       case MB200_RED_PROD: MB_RED(MB200_RED_PROD, double)
       case MB200_RED_SSD: MB_RED(MB200_RED_SSD, double)
+      case MB200_RED_ARGMIN: MB_RED(MB200_RED_ARGMIN, double)
+      case MB200_RED_ARGMAX: MB_RED(MB200_RED_ARGMAX, double)
     }
   } else if (dtype == MB200_I64) {
     switch (op) {
@@ -576,6 +736,8 @@ static int reduce_columns_impl(int op, int dtype, int ncols, const void* const* 
       case MB200_RED_MAX: MB_RED(MB200_RED_MAX, long long)
       case MB200_RED_COUNT: MB_RED(MB200_RED_COUNT, long long)
       case MB200_RED_PROD: MB_RED(MB200_RED_PROD, long long)
+      case MB200_RED_ARGMIN: MB_RED(MB200_RED_ARGMIN, long long)
+      case MB200_RED_ARGMAX: MB_RED(MB200_RED_ARGMAX, long long)
     }
   }
 #undef MB_RED

@@ -995,6 +995,137 @@ class DevVar(DevFn):
         return self(block, *args, **kwargs)
 
 
+_LABEL_EMPTY, _LABEL_I64, _LABEL_F64, _LABEL_REFUSED = 0, 1, 2, 3
+
+
+class DevArgReduce(DevFn):
+    """``pandas.DataFrame.idxmax / idxmin`` of one FULL column partition -> 1 x W block of row labels: the device body
+    of the Reduce template (alg/reduce.py:32-71; qc.py:1101-1102 registers ``Reduce.register(pandas.DataFrame.idxmax
+    / idxmin)``).
+
+    One pass over the block (``mb200_reduce_arg_columns``) gives per column the extreme value, the first row holding it
+    and the number of non-NaN values; the row becomes its label on the device (range start + row, or a gather from the
+    device index column) and the counts decide pandas' errors.  When the rows are sharded over ranks every rank
+    all-gathers its (value, label, count) W-vectors plus its row count -- one collective -- and combines them in rank
+    order: the better value wins and a tie goes to the lower rank, which holds the earlier rows.  Ranks without a
+    valid value in a column do not take part in it, and the errors are decided from the job-wide counts, so every rank
+    raises the same error after the same collective.  Labels are int64 (range or int64 index) or float64; string
+    labels, several index levels and ``axis=1`` are refused."""
+
+    def __init__(self, op: str):
+        if op not in ("max", "min"):
+            raise ValueError(op)
+        self.op = op
+
+    @staticmethod
+    def _label_kind(block):
+        """(kind code, refusal message) of the block's row labels."""
+        if block.nrows == 0:
+            return _LABEL_EMPTY, None
+        if block.has_range_index():
+            return _LABEL_I64, None
+        if block.index_cols:
+            if len(block.index_cols) != 1:
+                return _LABEL_REFUSED, "idxmax / idxmin over several index levels is not on the B200 path"
+            return (_LABEL_F64 if block.index_cols[0].dtype == np.float64 else _LABEL_I64), None
+        idx = block.index_host
+        if isinstance(idx, pandas.MultiIndex):
+            return _LABEL_REFUSED, "idxmax / idxmin over several index levels is not on the B200 path"
+        if idx.dtype.kind not in "if":
+            return _LABEL_REFUSED, f"idxmax / idxmin over {idx.dtype} row labels is not on the B200 path"
+        return (_LABEL_F64 if idx.dtype.kind == "f" else _LABEL_I64), None
+
+    @staticmethod
+    def _labels(block, kind, pos):
+        """Row labels at the W positions ``pos`` (int64 device tensor; -1 gives an arbitrary label)."""
+        t = ops.torch_mod()
+        if kind == _LABEL_EMPTY:
+            return t.zeros_like(pos)
+        p = DeviceColumn(pos, np.int64)
+        if block.has_range_index():
+            return ops.map_columns("add_s", [p], s0=[block.range_start])[0].data
+        if block.index_cols:
+            return ops.take_columns([block.index_cols[0]], p)[0].data
+        host = block.index_host.to_numpy().astype(np.float64 if kind == _LABEL_F64 else np.int64)
+        at = pos.tolist()
+        return t.tensor([host[i] if i >= 0 else 0 for i in at], dtype=t.float64 if kind == _LABEL_F64 else t.int64,
+                        device=pos.device)  # fmt: skip
+
+    def _raise_for(self, counts, nrows, skipna):
+        """pandas' errors (nanops._maybe_arg_null_out and the empty check), from the counts of the whole axis."""
+        if nrows == 0:
+            raise ValueError(f"attempt to get arg{self.op} of an empty sequence")
+        if skipna and min(counts) == 0:
+            raise ValueError("Encountered all NA values")
+        if not skipna and min(counts) < nrows:
+            raise ValueError("Encountered an NA value with skipna=False")
+
+    def __call__(self, block, *args, axis=0, skipna=True, numeric_only=False, **kwargs):
+        _check_block(block, f"DevArgReduce({self.op})")
+        if axis not in (0, "index", None) or args:
+            raise NotImplementedError(f"row-wise idx{self.op} (axis=1) is not on the B200 path")
+        if not block.cols:
+            return _reduced_block([], block.columns)
+        spans = _spans_ranks(block)
+        kind, refusal = self._label_kind(block)
+        if refusal and not spans:
+            raise NotImplementedError(refusal)
+        t = ops.torch_mod()
+        W = len(block.cols)
+        cols = ops.cast_columns_i64(block.cols)
+        vals, poss, cnts = ops.arg_reduce_columns(self.op, cols, ReduceVariant.get())
+        pos = t.cat([p.reshape(1) for p in poss])
+        cnt = t.cat([c.reshape(1) for c in cnts])
+        labels = self._labels(block, kind, pos) if not refusal else t.zeros_like(pos)
+        nrows = block.nrows
+        if spans:
+            labels, cnt, nrows, kind = self._combine_ranks(vals, labels, cnt, nrows, kind, cols)
+        host = t.cat([cnt, t.full((1,), nrows, dtype=t.int64, device=cnt.device)]).tolist()  # one D2H
+        self._raise_for(host[:W], host[W], bool(skipna))
+        dtype = np.float64 if kind == _LABEL_F64 else np.int64
+        out = [DeviceColumn(labels[j : j + 1], dtype) for j in range(W)]
+        res = _reduced_block(out, block.columns)
+        res.replicated = spans
+        return res
+
+    def run_distributed(self, block, *args, **kwargs):
+        return self(block, *args, **kwargs)
+
+    def _combine_ranks(self, vals, labels, cnt, nrows, kind, cols):
+        """All-gather (value bits, label bits, count) per column and (rows, label kind) per rank, combine in rank
+        order.  Returns the job-wide (labels, counts, rows, label kind); raises on every rank alike."""
+        from . import dist
+
+        t = ops.torch_mod()
+        W = len(cols)
+        bits = lambda x: x.view(t.int64) if x.dtype == t.float64 else x  # noqa: E731
+        vb = t.cat([bits(v.reshape(1)) for v in vals])
+        meta = t.tensor([nrows, kind], dtype=t.int64, device=vb.device)
+        g = dist.all_gather_fixed(t.cat([vb, bits(labels), cnt, meta])).view(-1, 3 * W + 2)
+        rank_meta = g[:, 3 * W :].tolist()  # [rows, label kind] per rank
+        kinds = {k for _, k in rank_meta} - {_LABEL_EMPTY}
+        if _LABEL_REFUSED in kinds or len(kinds) > 1:
+            raise NotImplementedError("idxmax / idxmin on the B200 path need int64 or float64 row labels of one kind "
+                                      "on every rank")  # fmt: skip
+        is_f = t.tensor([c.dtype == np.float64 for c in cols], device=vb.device)
+        v_i, lab, cn = g[:, :W].contiguous(), g[:, W : 2 * W].contiguous(), g[:, 2 * W : 3 * W]
+        v_f = v_i.view(t.float64)
+        best_i, best_f, best_l, have = v_i[0], v_f[0], lab[0], cn[0] > 0
+        for r in range(1, g.shape[0]):
+            ok = cn[r] > 0
+            if self.op == "max":
+                better = t.where(is_f, v_f[r] > best_f, v_i[r] > best_i)
+            else:
+                better = t.where(is_f, v_f[r] < best_f, v_i[r] < best_i)
+            take = ok & (~have | better)  # strict: a tie stays with the lower rank
+            best_i, best_f = t.where(take, v_i[r], best_i), t.where(take, v_f[r], best_f)
+            best_l = t.where(take, lab[r], best_l)
+            have = have | ok
+        kind = kinds.pop() if kinds else _LABEL_I64
+        out = best_l.view(t.float64) if kind == _LABEL_F64 else best_l
+        return out, cn.sum(0), sum(n for n, _ in rank_meta), kind
+
+
 # ------------------------------------------------------------------ Fold functor
 class DevCumulative(DevFn):
     """``pandas.DataFrame.cumsum / cummax / cummin`` (qc.py:2429-2431) and ``DataFrame.ffill`` (``fillna(method=

@@ -675,6 +675,10 @@ def register(shims: bool | None = None):
 
         # qc.py:1155-1156: std / var = Reduce.register(pandas.DataFrame.std / var) -- same template, device functor
         # (two sweeps over each full column partition, two packed all-reduces when the rows span ranks)
+        # qc.py:1101-1102: idxmax / idxmin = Reduce.register(pandas.DataFrame.idxmax / idxmin) -- one arg-reduction
+        # pass per column partition, one W-vector all-gather when the rows span ranks
+        idxmax = Reduce.register(fx.DevArgReduce("max"))
+        idxmin = Reduce.register(fx.DevArgReduce("min"))
         var = Reduce.register(fx.DevVar(sqrt=False))
         std = Reduce.register(fx.DevVar(sqrt=True))
         # qc.py:2429-2431: cumulative functions through the Fold template (csrc/cum.cu); forward fill rides the same

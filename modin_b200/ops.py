@@ -220,6 +220,40 @@ def reduce_columns(op: str, cols: Sequence[DeviceColumn], skipna: bool = True, v
     return vals, cnts
 
 
+def arg_reduce_columns(op: str, cols: Sequence[DeviceColumn], variant: int = 0):
+    """Column-wise extreme value and the first row holding it (``op`` "max" / "min"; idxmax / idxmin) in one pass.
+
+    Returns ``(vals, poss, cnts)``, 1-element device views per column in column order: the extreme value in the
+    column's dtype, its row position (-1 when the column holds no valid value) and the number of non-NaN values.
+    float64 / int64 columns; 8 columns per launch, like ``reduce_columns``."""
+    lib = _lib.load()
+    t = torch_mod()
+    code_op = _lib.RED["arg" + op]
+    n = len(cols[0]) if cols else 0
+    vals: list = [None] * len(cols)
+    poss: list = [None] * len(cols)
+    cnts: list = [None] * len(cols)
+    groups = {}
+    for j, c in enumerate(cols):
+        groups.setdefault(c.code, []).append(j)
+    for code, idxs in groups.items():
+        if code == _lib.U8:
+            raise TypeError("arg-reductions over bool columns are not on the B200 path (widen them to int64)")
+        for k in range(0, len(idxs), 8):
+            sel = idxs[k : k + 8]
+            oval = t.empty(len(sel), dtype=t.float64 if code == _lib.F64 else t.int64, device=current_device())
+            opos = t.empty(len(sel), dtype=t.int64, device=current_device())
+            ocnt = t.empty(len(sel), dtype=t.int64, device=current_device())
+            scratch = _scratch(lib.mb200_reduce_scratch_bytes(len(sel)), "reduce")
+            with _timed("reduce_arg" + op):
+                _lib.check(lib.mb200_reduce_arg_columns(code_op, code, len(sel), _lib.ptr_array([cols[j].ptr for j in sel]),
+                                                        n, oval.data_ptr(), opos.data_ptr(), ocnt.data_ptr(),
+                                                        scratch.data_ptr(), variant, current_stream()))  # fmt: skip
+            for pos, j in enumerate(sel):
+                vals[j], poss[j], cnts[j] = oval[pos : pos + 1], opos[pos : pos + 1], ocnt[pos : pos + 1]
+    return vals, poss, cnts
+
+
 # ------------------------------------------------------------------ GroupByReduce
 class GroupTable:
     """Owner of one device hash table (mb200_gb_table)."""

@@ -255,6 +255,20 @@ class BasePandasDataset:
             raise NotImplementedError("count(axis=1) is not on the B200 path")
         return self._reduce_dimension(self._query_compiler.count(axis=0, numeric_only=numeric_only))
 
+    # ---- Reduce: label of the first extreme value (modin/pandas/base.py ``idxmax`` / ``idxmin``) ----------------
+    def _arg_stat(self, name, axis, skipna, numeric_only):
+        if axis not in (0, "index", None):
+            raise NotImplementedError(f"{name}(axis=1) is not on the B200 path")
+        if not len(self._query_compiler.columns):
+            return pandas.Series([], index=self._query_compiler.columns, dtype=np.int64)
+        return self._reduce_dimension(getattr(self._query_compiler, name)(axis=0, skipna=skipna, numeric_only=numeric_only))
+
+    def idxmax(self, axis=0, skipna=True, numeric_only=False):
+        return self._arg_stat("idxmax", axis, skipna, numeric_only)
+
+    def idxmin(self, axis=0, skipna=True, numeric_only=False):
+        return self._arg_stat("idxmin", axis, skipna, numeric_only)
+
     # ---- misc --------------------------------------------------------------------------------------
     def _to_pandas(self):
         return self._query_compiler.to_pandas()
@@ -527,6 +541,19 @@ class Series(BasePandasDataset):
             raise NotImplementedError("Series.rename on the B200 path only changes the name")
         label = MODIN_UNNAMED_SERIES_LABEL if index is None else index
         return Series(query_compiler=self._query_compiler.relabel_columns([label]))
+
+    def argmax(self, axis=None, skipna=True, *args, **kwargs):
+        """Position of the first largest value: ``idxmax`` over the rows renumbered 0..n-1, as modin/pandas/series.py
+        ``argmax`` does with ``reset_index(drop=True)`` (metadata only, no copy)."""
+        return self._positions().idxmax(skipna=skipna)
+
+    def argmin(self, axis=None, skipna=True, *args, **kwargs):
+        return self._positions().idxmin(skipna=skipna)
+
+    def _positions(self) -> "Series":
+        from ..query_compiler import _reset_row_index
+
+        return Series(query_compiler=self._query_compiler.__constructor__(_reset_row_index(self._query_compiler._modin_frame)))
 
     def __getitem__(self, key):
         """``s[bool_series]``: boolean row selection, as on a frame."""

@@ -20,6 +20,7 @@ import pandas
 from .algebra import Binary, Fold, GroupByReduce, Map, Reduce, TreeReduce
 from .dataframe import B200Dataframe
 from .functors import (
+    DevArgReduce,
     DevAstype,
     DevBinary,
     DevBoolReduce,
@@ -246,6 +247,9 @@ class B200QueryCompiler:
                               compute_dtypes=lambda *a, **k: np.dtype("bool"))  # qc.py:987
 
     # ---- Reduce (qc.py:1155-1156: std / var = Reduce.register(pandas.DataFrame.std / var)) ---------------------------
+    # qc.py:1101-1102: idxmax / idxmin = Reduce.register(pandas.DataFrame.idxmax / idxmin) -- one arg-reduction pass
+    idxmax = Reduce.register(DevArgReduce("max"))
+    idxmin = Reduce.register(DevArgReduce("min"))
     _var_frame = Reduce.register(DevVar(sqrt=False))
     _std_frame = Reduce.register(DevVar(sqrt=True))
 
