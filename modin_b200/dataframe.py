@@ -185,7 +185,7 @@ class B200Dataframe:
 
     def tree_reduce(self, axis, map_func: Callable, reduce_func: Optional[Callable] = None, dtypes=None):
         """df.py:2208-2250: map every block to a 1 x W partial, then reduce each column partition's
-        partials (plus an all_reduce across GPUs, issued by the reduce functor's collective hook)."""
+        partials (plus an all_reduce across GPUs, issued by the reduce-phase functor itself)."""
         if axis != 0:
             raise NotImplementedError("tree_reduce along axis=1 is not on the B200 path")
         map_func = self._build_treereduce_func(axis, map_func)

@@ -15,7 +15,7 @@ silent pandas fallback on this path.
 from __future__ import annotations
 
 import numbers
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import numpy as np
 import pandas
@@ -558,13 +558,13 @@ class DevDropDuplicates(DevFn):
     def __call__(self, block, key_position=0, keep="first", ignore_index=False, **kwargs):
         _check_block(block, "DevDropDuplicates")
         if _spans_ranks(block):
-            return self.run_distributed(block, key_position, keep=keep, ignore_index=ignore_index)
+            return self._across_ranks(block, key_position, keep, ignore_index)
         self._validate(block, key_position, keep, ignore_index)
         if block.nrows <= 1:
             return DeviceBlock(block.cols, block.columns, nrows=block.nrows, range_start=0) if ignore_index else block
         return self._rows(block, self._winners(block.cols[key_position], keep), ignore_index, 0)
 
-    def run_distributed(self, block, key_position=0, keep="first", ignore_index=False, **kwargs):
+    def _across_ranks(self, block, key_position, keep, ignore_index):
         """Rows sharded over ranks: equal keys may sit on different GPUs, so a shard-local answer is not the answer.
         Every rank finds its own first / last occurrence per key; only the KEYS of those survivors (one int64 per
         rank and distinct key) are all-gathered, in rank order -- which is row order, shards are contiguous; the
@@ -572,7 +572,6 @@ class DevDropDuplicates(DevFn):
         from its own survivors.  The result stays row-sharded and in row order like any other frame; no row moves."""
         from . import dist
 
-        _check_block(block, "DevDropDuplicates")
         self._validate(block, key_position, keep, ignore_index)
         t = ops.torch_mod()
         key = block.cols[key_position]
@@ -675,22 +674,16 @@ class DevBoolReduce(DevFn):
         return _reduced_block(ops.map_columns("gt_s", ints, s0=[0] * len(ints)), block.columns)
 
     def __call__(self, block, *args, axis=0, skipna=True, **kwargs):
+        from . import dist
+
         _check_block(block, f"DevBoolReduce({self.op})")
         if axis not in (0, "index", None):
             raise NotImplementedError("row-wise any / all is not on the B200 path")
-        if self.phase == "reduce" and _spans_ranks(block):
-            return self.run_distributed(block, *args, axis=axis, skipna=skipna, **kwargs)
         if not block.cols:
             return _reduced_block([], block.columns)
         vals, _ = ops.reduce_columns(self.kop, self._ints(block), skipna=True, variant=1)
-        return self._finish(vals, block)
-
-    def run_distributed(self, block, *args, axis=0, skipna=True, **kwargs):
-        from . import dist
-
-        if not block.cols:
-            return _reduced_block([], block.columns)
-        vals, _ = ops.reduce_columns(self.kop, self._ints(block), skipna=True, variant=1)
+        if self.phase != "reduce" or not _spans_ranks(block):
+            return self._finish(vals, block)
         dist.all_reduce_values(vals, [self.kop] * len(vals))
         res = self._finish(vals, block)
         res.replicated = True
@@ -785,14 +778,14 @@ class DevReduce(DevFn):
 
     def __call__(self, block, *args, axis=0, skipna=True, numeric_only=False, min_count=0, **kwargs):
         self._check(block, axis, min_count)
-        if self.phase == "reduce" and _spans_ranks(block):
-            return self.run_distributed(block, *args, axis=axis, skipna=skipna, numeric_only=numeric_only,
-                                        min_count=min_count, **kwargs)  # fmt: skip
         if not block.cols:
             return _reduced_block([], block.columns)
+        spans = self.phase == "reduce" and _spans_ranks(block)
         kop = self._kernel_op()
         block = self._widen_bools(block, kop)
         vals, cnts = ops.reduce_columns(kop, block.cols, skipna=bool(skipna), variant=ReduceVariant.get())
+        if spans:
+            return self._across_ranks(block, kop, vals, cnts, skipna, min_count)
         out = []
         for j, c in enumerate(block.cols):
             if kop == "count":
@@ -807,19 +800,14 @@ class DevReduce(DevFn):
         res.replicated = block.replicated  # a partial of rows every rank holds in full is such a partial too
         return res
 
-    def run_distributed(self, block, *args, axis=0, skipna=True, numeric_only=False, min_count=0, **kwargs):
-        """Reduce-phase body when rows are sharded over several GPUs: local reduction of this rank's
-        partials, then ONE packed all_reduce of the W-vector (sum / min / max) -- the collective that
-        replaces the reference's gather-to-one-task (axis_partition.py:445-452)."""
+    @staticmethod
+    def _across_ranks(block, kop, vals, cnts, skipna, min_count):
+        """Reduce phase when rows are sharded over several GPUs: this rank's reduction of its partials (``vals`` /
+        ``cnts``) goes into ONE packed all_reduce of the W-vector (sum / min / max) -- the collective that replaces
+        the reference's gather-to-one-task (axis_partition.py:445-452)."""
         from . import dist
 
-        self._check(block, axis, min_count)
-        if not block.cols:
-            return _reduced_block([], block.columns)
         t = ops.torch_mod()
-        kop = self._kernel_op()
-        block = self._widen_bools(block, kop)
-        vals, cnts = ops.reduce_columns(kop, block.cols, skipna=bool(skipna), variant=ReduceVariant.get())
         W = len(block.cols)
         if kop == "count":
             dist.all_reduce_values(cnts, ["sum"] * W)
@@ -932,17 +920,13 @@ class DevMeanReduce(DevFn):
         return _reduced_block(ops.map_columns("div", s, c), labels)
 
     def __call__(self, block, *args, axis=0, skipna=True, **kwargs):
-        _check_block(block, "DevMeanReduce")
-        if _spans_ranks(block):
-            return self.run_distributed(block, *args, axis=axis, skipna=skipna, **kwargs)
-        return self._divide(*self._local(block))
-
-    def run_distributed(self, block, *args, axis=0, skipna=True, **kwargs):
-        """Sums and counts are all_reduced BEFORE the division (mean of shard means would be wrong)."""
         from . import dist
 
         _check_block(block, "DevMeanReduce")
         sums, cnts, labels = self._local(block)
+        if not _spans_ranks(block):
+            return self._divide(sums, cnts, labels)
+        # across ranks, sums and counts are all_reduced BEFORE the division (mean of shard means would be wrong)
         dist.all_reduce_values(sums + cnts, ["sum"] * (len(sums) + len(cnts)))
         res = self._divide(sums, cnts, labels)
         res.replicated = True
@@ -990,9 +974,6 @@ class DevVar(DevFn):
         res = _reduced_block([DeviceColumn(out[j : j + 1], np.float64) for j in range(W)], block.columns)
         res.replicated = spans
         return res
-
-    def run_distributed(self, block, *args, **kwargs):
-        return self(block, *args, **kwargs)
 
 
 _LABEL_EMPTY, _LABEL_I64, _LABEL_F64, _LABEL_REFUSED = 0, 1, 2, 3
@@ -1088,9 +1069,6 @@ class DevArgReduce(DevFn):
         res.replicated = spans
         return res
 
-    def run_distributed(self, block, *args, **kwargs):
-        return self(block, *args, **kwargs)
-
     def _combine_ranks(self, vals, labels, cnt, nrows, kind, cols):
         """All-gather (value bits, label bits, count) per column and (rows, label kind) per rank, combine in rank
         order.  Returns the job-wide (labels, counts, rows, label kind); raises on every rank alike."""
@@ -1153,9 +1131,6 @@ class DevCumulative(DevFn):
         if self.op == "ffill" and (kwargs.get("limit") is not None or kwargs.get("limit_area") is not None):
             raise NotImplementedError("ffill(limit=) is not on the B200 path")
         return self._run(block, _spans_ranks(block))
-
-    def run_distributed(self, block, *args, **kwargs):
-        return self(block, *args, **kwargs)
 
     def _run(self, block, distributed: bool):
         from . import dist
@@ -1285,14 +1260,39 @@ class DevReindex(DevFn):
 
 
 # ------------------------------------------------------------------ GroupByReduce functors
-_GB_FLAGS = {
-    "min": _lib.GB_MIN,
-    "max": _lib.GB_MAX,
-    "sum": _lib.GB_SUM,
-    "count": _lib.GB_COUNT,
-    "size": _lib.GB_SIZE,
-    "mean": _lib.GB_SUM | _lib.GB_COUNT,
+class _Partial(NamedTuple):
+    """What a partial group table of one aggregation carries: the table flags, and the emitted arrays in column order
+    (``sums`` / ``cnts``: one column per value column, under the value labels -- or under ``("sum", label)`` /
+    ``("count", label)`` when there are both; ``sizes``: one column labelled "size")."""
+
+    flags: int
+    arrays: tuple
+
+
+_PARTIALS = {
+    "min": _Partial(_lib.GB_MIN, ("sums",)),
+    "max": _Partial(_lib.GB_MAX, ("sums",)),
+    "sum": _Partial(_lib.GB_SUM, ("sums",)),
+    "count": _Partial(_lib.GB_COUNT, ("cnts",)),
+    "size": _Partial(_lib.GB_SIZE, ("sizes",)),
+    "mean": _Partial(_lib.GB_SUM | _lib.GB_COUNT, ("sums", "cnts")),  # mean = sums / counts, in _finished_block
 }
+
+
+def _partial_cols(agg, sums, cnts, sizes):
+    """The emitted arrays of a table in the partial layout of ``agg``."""
+    got = {"sums": sums, "cnts": cnts, "sizes": [sizes]}
+    return [c for name in _PARTIALS[agg].arrays for c in got[name]]
+
+
+def _partial_labels(agg, labels):
+    arrays = _PARTIALS[agg].arrays
+    if arrays == ("sizes",):
+        return pandas.Index(["size"])
+    if len(arrays) == 1:
+        return labels
+    tags = {"sums": "sum", "cnts": "count"}
+    return pandas.MultiIndex.from_tuples([(tags[name], c) for name in arrays for c in labels])
 
 
 _VALUE_POSITIONS: dict = {}
@@ -1313,20 +1313,53 @@ def _value_positions(columns: pandas.Index, key_label):
     return keep, labels
 
 
-def _split_key_values(block: DeviceBlock, by_block: Optional[DeviceBlock]):
-    """Key column + value columns of one row block (alg/groupby.py:186-206: with drop=True the
-    `by` column is taken out of the data, or concatenated in when it lives in another frame)."""
+def _split_key_values(block: DeviceBlock, by_block: Optional[DeviceBlock], who: str):
+    """Key column, its label, value columns and their labels of one row block (alg/groupby.py:186-206: with
+    drop=True the `by` column is taken out of the data, or concatenated in when it lives in another frame)."""
+    _check_block(block, who)
     if by_block is None:
         raise NotImplementedError("groupby needs a `by` block on the B200 path")
     if len(by_block.cols) != 1:
         raise NotImplementedError("multi-column `by` is not on the B200 path yet")
     key = by_block.cols[0]
-    key_label = by_block.columns[0]
-    keep, labels = _value_positions(block.columns, key_label)
-    vals = [block.cols[i] for i in keep]
+    keep, labels = _value_positions(block.columns, by_block.columns[0])
     if key.dtype != np.int64:
         raise NotImplementedError("device groupby needs an int64 key column")
-    return key, key_label, vals, labels
+    return key, by_block.columns[0], [block.cols[i] for i in keep], labels
+
+
+def _aggregated_values(agg, vals):
+    """The value columns ``agg`` aggregates: none for size, float64 images for count / mean (the table counts non-NaN
+    float64 values); the others take float64 columns only."""
+    if agg == "size":
+        return []
+    vals = ops.cast_columns_f64(vals) if agg in ("count", "mean") else vals
+    if any(v.dtype != np.float64 for v in vals):
+        raise NotImplementedError(f"device groupby.{agg} aggregates float64 value columns only")
+    return vals
+
+
+def _group_block(cols, labels, keys, key_label, count_dev=None):
+    """One row per group, ascending by key (the device index column).  With ``count_dev`` the columns have room for
+    more rows than there are groups; the count stays on the device until it is read."""
+    if count_dev is not None:
+        blk = DeviceBlock.with_device_count(cols, labels, count_dev, index_cols=[keys], index_names=[key_label],
+                                            check=ops.refuse_dense_overflow)  # fmt: skip
+    else:
+        blk = DeviceBlock(cols, labels, nrows=len(keys), index_cols=[keys], index_names=[key_label])
+    blk.keys_sorted_unique = True
+    return blk
+
+
+def _finished_block(agg, keys, key_label, cols, labels):
+    """The groupby result from merged partial columns ``cols`` (the layout of ``agg``); ``labels`` are the value
+    labels.  A mean divides its sums by its counts."""
+    if agg == "mean":
+        W = len(cols) // 2
+        cf = ops.cast_columns_f64(cols[W:])
+        cols = ops.map_columns("div", cols[:W], cf) if len(keys) else cols[:W]
+        return _group_block(cols, labels, keys, key_label)
+    return _group_block(cols, _partial_labels(agg, labels), keys, key_label)
 
 
 class DevGroupbyMap(DevFn):
@@ -1334,43 +1367,17 @@ class DevGroupbyMap(DevFn):
     slice of `by` into a partial table (index = keys, ascending)."""
 
     def __init__(self, agg: str, capacity_hint: int = 1 << 20):
-        if agg not in _GB_FLAGS:
+        if agg not in _PARTIALS:
             raise NotImplementedError(f"groupby.{agg} is not on the B200 path")
         self.agg = agg
         self.op = f"groupby_{agg}_map"
         self.capacity_hint = capacity_hint
 
     def __call__(self, block, by_block=None, *args, **kwargs):
-        _check_block(block, self.op)
-        key, key_label, vals, labels = _split_key_values(block, by_block)
-        flags = _GB_FLAGS[self.agg]
-        if self.agg == "size":
-            vals, labels = [], labels[:0]
-        else:
-            vals = ops.cast_columns_f64(vals) if self.agg in ("count", "mean") else vals
-            if any(v.dtype != np.float64 for v in vals):
-                raise NotImplementedError(f"device groupby.{self.agg} aggregates float64 value columns only")
-        cap = max(1024, min(self.capacity_hint, block.nrows))
-        keys, sums, cnts, sizes = ops.hash_aggregate([(key, vals)], flags, cap)
-        return _partial_block(self.agg, keys, key_label, sums, cnts, sizes, labels)
-
-
-def _partial_block(agg, keys, key_label, sums, cnts, sizes, labels, count_dev=None, check=None):
-    if agg in ("sum", "min", "max"):
-        cols, cl = sums, labels
-    elif agg == "count":
-        cols, cl = cnts, labels
-    elif agg == "size":
-        cols, cl = [sizes], pandas.Index(["size"])
-    else:  # mean: sums then counts
-        cols = list(sums) + list(cnts)
-        cl = pandas.MultiIndex.from_tuples([("sum", c) for c in labels] + [("count", c) for c in labels])
-    if count_dev is not None:
-        blk = DeviceBlock.with_device_count(cols, cl, count_dev, index_cols=[keys], index_names=[key_label], check=check)
-    else:
-        blk = DeviceBlock(cols, cl, nrows=len(keys), index_cols=[keys], index_names=[key_label])
-    blk.keys_sorted_unique = True
-    return blk
+        key, key_label, vals, labels = _split_key_values(block, by_block, self.op)
+        vals = _aggregated_values(self.agg, vals)
+        keys, sums, cnts, sizes = ops.hash_aggregate([(key, vals)], _PARTIALS[self.agg].flags, self.capacity_hint)
+        return _group_block(_partial_cols(self.agg, sums, cnts, sizes), _partial_labels(self.agg, labels), keys, key_label)
 
 
 def keys_to_columns(block: DeviceBlock, offset: int = 0) -> DeviceBlock:
@@ -1396,72 +1403,44 @@ class DevGroupbyReduce(DevFn):
         self.op = f"groupby_{agg}_reduce"
 
     def _merge(self, keys, cols):
-        """Regroup partial rows by key -> ascending unique keys + merged partial columns (same layout
-        as the input: sums | counts | size, depending on the aggregation)."""
-        agg = self.agg
-        n = len(keys)
-        if agg in ("sum", "min", "max"):  # partial sums add up; partial minima / maxima reduce with min / max
-            k, s, _, _ = ops.hash_aggregate([(keys, cols, None, None)], _GB_FLAGS[agg], n, partial=True)
-            return k, list(s)
-        if agg == "count":
-            # int64 partial counts are merged through the count accumulators (values are ignored)
-            dummy = [ops.cast_columns_f64([c])[0] for c in cols]
-            k, _, c, _ = ops.hash_aggregate([(keys, dummy, cols, None)], _lib.GB_COUNT, n, partial=True)
-            return k, list(c)
-        if agg == "size":
-            k, _, _, z = ops.hash_aggregate([(keys, [], None, cols[0])], _lib.GB_SIZE, n, partial=True)
-            return k, [z]
-        W = len(cols) // 2
-        k, s, c, _ = ops.hash_aggregate([(keys, cols[:W], cols[W:], None)], _lib.GB_SUM | _lib.GB_COUNT, n,
-                                        partial=True)  # fmt: skip
-        return k, list(s) + list(c)
+        """Regroup partial rows by key -> ascending unique keys + merged partial columns (same layout as the input).
+        Partial sums add up, partial minima / maxima reduce with min / max, counts and sizes add up."""
+        layout = _PARTIALS[self.agg]
+        W = len(cols) // len(layout.arrays)
+        got = {name: list(cols[i * W : (i + 1) * W]) for i, name in enumerate(layout.arrays)}
+        sums, cnts, sizes = got.get("sums"), got.get("cnts"), got.get("sizes", [None])[0]
+        if sums is None:
+            # partial counts are merged through the count accumulators, which want value columns (ignored)
+            sums = ops.cast_columns_f64(cnts) if cnts is not None else []
+        k, s, c, z = ops.hash_aggregate([(keys, sums, cnts, sizes)], layout.flags, len(keys), partial=True)
+        return k, _partial_cols(self.agg, s, c, z)
 
     def _finalize(self, k, cols, columns, key_label):
-        if self.agg == "mean":
-            W = len(cols) // 2
-            cf = ops.cast_columns_f64(cols[W:])
-            labels = pandas.Index([t[1] for t in columns[:W]])
-            return DeviceBlock(ops.map_columns("div", cols[:W], cf) if len(k) else cols[:W], labels, nrows=len(k),
-                               index_cols=[k], index_names=[key_label])  # fmt: skip
-        return DeviceBlock(cols, columns, nrows=len(k), index_cols=[k], index_names=[key_label])
+        labels = pandas.Index([t[1] for t in columns[: len(cols) // 2]]) if self.agg == "mean" else columns
+        return _finished_block(self.agg, k, key_label, cols, labels)
 
-    def _unpack(self, block):
+    def __call__(self, block, *args, partition_idx=0, **kwargs):
         _check_block(block, self.op)
         if not block.index_cols:
             raise ValueError("groupby reduce expects partial tables keyed by device index columns")
-        return block.index_cols[0], (block.index_names[0] if block.index_names else None)
-
-    def _local_merge(self, block, keys):
+        keys, key_label = block.index_cols[0], (block.index_names[0] if block.index_names else None)
         # a single partial table (one row partition on this GPU) is already one row per key, ascending:
         # nothing to regroup -- the reference would re-run groupby(level=0) on it to the same effect
-        if block.keys_sorted_unique:
-            return keys, list(block.cols)
-        return self._merge(keys, block.cols)
-
-    def __call__(self, block, *args, partition_idx=0, **kwargs):
+        k, cols = (keys, list(block.cols)) if block.keys_sorted_unique else self._merge(keys, block.cols)
         if _spans_ranks(block):
-            return self.run_distributed(block, *args, partition_idx=partition_idx, **kwargs)
-        keys, key_label = self._unpack(block)
-        k, cols = self._local_merge(block, keys)
+            k, cols = self._across_ranks(k, cols)
         return self._finalize(k, cols, block.columns, key_label)
 
-    def run_distributed(self, block, *args, partition_idx=0, **kwargs):
-        """The groupby shuffle: merge this rank's partial tables, range-partition the merged table by
-        key over the ranks (all-to-all of <= G pre-aggregated rows per GPU, never raw rows), merge
-        what arrives.  Rank r ends up owning the r-th key range, ascending -- the concatenation over
-        ranks is the reference's key-sorted result."""
+    def _across_ranks(self, k, cols):
+        """The groupby shuffle: range-partition this rank's merged table by key over the ranks (all-to-all of <= G
+        pre-aggregated rows per GPU, never raw rows) and merge what arrives.  Rank r ends up owning the r-th key
+        range, ascending -- the concatenation over ranks is the reference's key-sorted result."""
         from . import dist
 
-        keys, key_label = self._unpack(block)
-        k, cols = self._local_merge(block, keys)
         rk, rcols = dist.exchange_by_key_range(k.data, [c.data for c in cols])
         rkeys = DeviceColumn(rk, np.int64)
         rc = [DeviceColumn(t_, c.dtype) for t_, c in zip(rcols, cols)]
-        if len(rkeys):
-            k2, cols2 = self._merge(rkeys, rc)
-        else:
-            k2, cols2 = rkeys, rc
-        return self._finalize(k2, cols2, block.columns, key_label)
+        return self._merge(rkeys, rc) if len(rkeys) else (rkeys, rc)
 
 
 def fused_dense_groupby(map_fn: "DevGroupbyMap", reduce_fn: "DevGroupbyReduce", blocks, by_blocks):
@@ -1472,86 +1451,41 @@ def fused_dense_groupby(map_fn: "DevGroupbyMap", reduce_fn: "DevGroupbyReduce", 
 
     Returns the finished result block, or None when the keys are not dense-able (the caller then runs
     the general map -> exchange -> reduce path).  Every rank takes the same decision: it is made on the
-    all-reduced key range and row count."""
+    job-wide key range and row count (``ops.plan_table``)."""
     from . import dist
-    from .config import GroupbyAsyncEmit, GroupbyDenseKeys
+    from .config import GroupbyAsyncEmit
 
-    if not GroupbyDenseKeys.get() or map_fn.agg != reduce_fn.agg or not blocks or len(blocks) != len(by_blocks):
-        return None
     agg = map_fn.agg
-    flags = _GB_FLAGS[agg]
-    items, labels, key_label = [], None, None
-    for block, by_block in zip(blocks, by_blocks):
-        _check_block(block, map_fn.op)
-        key, key_label, vals, labels = _split_key_values(block, by_block)
-        if agg == "size":
-            vals, labels = [], labels[:0]
-        else:
-            vals = ops.cast_columns_f64(vals) if agg in ("count", "mean") else vals
-            if any(v.dtype != np.float64 for v in vals):
-                raise NotImplementedError(f"device groupby.{agg} aggregates float64 value columns only")
-        items.append((key, vals))
-    if len(labels) > _lib_max_cols():
+    if agg != reduce_fn.agg or not blocks or len(blocks) != len(by_blocks):
         return None
-    key_cols = [k for k, _ in items]
-    lo, hi, sampled, dup = ops.key_stats(key_cols)  # column metadata: no pass over the keys, no sync, once known
-    total_rows = sum(len(k) for k in key_cols)
-    if dist.is_distributed():
-        # every rank must take the same decision: job-wide range and row count, agreed on ONCE per set of key
-        # columns (one small all_gather + one D2H) and then remembered on the first of them -- columns are
-        # immutable and so is the job
-        sig = (dist.world_size(), tuple(id(k.data) for k in key_cols))
-        anchor = key_cols[0].stats
-        if anchor.job is None or anchor.job[0] != sig:
-            t = ops.torch_mod()
-            mine = t.tensor([lo, hi, total_rows], dtype=t.int64, device=ops.current_device())
-            trip = dist.all_gather_small(mine)
-            anchor.job = (sig, (min(r[0] for r in trip), max(r[1] for r in trip), sum(r[2] for r in trip)))
-        lo, hi, total_rows = anchor.job[1]  # `sampled` / `dup` stay local: the hot-group cache is a local choice
-    if lo > hi:
-        return None  # no rows anywhere
-    cap = max(1024, min(map_fn.capacity_hint, total_rows))
-    if not ops.dense_range_ok(lo, hi, cap, total_rows, len(labels), flags):
+    inputs = [_split_key_values(block, by_block, map_fn.op) for block, by_block in zip(blocks, by_blocks)]
+    key_label, labels = inputs[0][1], (inputs[0][3] if agg != "size" else inputs[0][3][:0])
+    if len(labels) > _lib.MAX_COLS:
         return None
-    ws = dist.world_size() if dist.is_distributed() else 1
-    # across GPUs the table spans the job-wide range padded to ws equal chunks, so that it can be reduce-scattered
-    chunk = dist.dense_chunk(hi - lo + 1, ws) if ws > 1 else 0
-    table = ops.GroupTable.dense(lo, lo + ws * chunk - 1 if ws > 1 else hi, len(labels), flags)
-    table.hint_skew(ops.keys_are_skewed(sampled, dup))
-    mine = None
+    plan = ops.plan_table([inp[0] for inp in inputs], len(labels), _PARTIALS[agg].flags, map_fn.capacity_hint,
+                          job_wide=True)  # fmt: skip
+    if plan is None:
+        return None
+    table, mine = plan.create(), None
     try:
-        for key, vals in items:
-            table.accumulate(key, vals)
-        if ws > 1:
+        ops.fill_table(table, [(key, _aggregated_values(agg, vals)) for key, _, vals, _ in inputs])
+        if plan.chunk:
             # the reduce phase: rank r receives the merged accumulators of ITS key slice only (no keys move,
             # no sort, no pivots) and emits it; the rank-ordered results are the reference's key-sorted frame
-            mine = table.reduce_scatter(chunk, dist.reduce_scatter, dist.rank())
+            mine = table.reduce_scatter(plan.chunk, dist.reduce_scatter, dist.rank())
         emitter = mine if mine is not None else table
         if agg != "mean" and GroupbyAsyncEmit.get():
             # no host round trip: the result block is sized on the device and learns its row count when somebody
             # asks (DeviceBlock.with_device_count) -- the host is free to prepare the next query meanwhile
             keys, sums, cnts, sizes, count = emitter.emit_async()
-
-            def check(vals):
-                if vals[1]:
-                    raise _lib.B200Error("dense group table saw a key outside its measured range")
-
-            part = _partial_block(agg, keys, key_label, sums, cnts, sizes, labels, count_dev=count, check=check)
-            return part
-        ng, overflow = emitter.ngroups()
-        if overflow:
-            raise _lib.B200Error("dense group table saw a key outside its measured range")
-        keys, sums, cnts, sizes = emitter.emit(ng, sort=False)
+            return _group_block(_partial_cols(agg, sums, cnts, sizes), _partial_labels(agg, labels), keys, key_label,
+                                count_dev=count)  # fmt: skip
+        keys, sums, cnts, sizes = ops.emit_counted(emitter, sort=False)
     finally:
         table.close()
         if mine is not None:
             mine.close()
-    part = _partial_block(agg, keys, key_label, sums, cnts, sizes, labels)
-    return reduce_fn._finalize(part.index_cols[0], list(part.cols), part.columns, key_label)
-
-
-def _lib_max_cols() -> int:
-    return 32  # MB200_MAX_COLS
+    return _finished_block(agg, keys, key_label, _partial_cols(agg, sums, cnts, sizes), labels)
 
 
 # ------------------------------------------------------------------ broadcast merge functor

@@ -9,7 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import List, Optional, Sequence
+from typing import List, NamedTuple, Optional, Sequence
 
 import numpy as np
 
@@ -255,8 +255,27 @@ def arg_reduce_columns(op: str, cols: Sequence[DeviceColumn], variant: int = 0):
 
 
 # ------------------------------------------------------------------ GroupByReduce
+_GB_ACC = _lib.GB_SUM | _lib.GB_MIN | _lib.GB_MAX
+_DENSE_ARRAYS = ("acc", "cnt", "size", "present")
+
+
+def value_stride(nvals: int) -> int:
+    """Accumulator slots per key of a dense table (include/modin_b200.h): ``nvals`` rounded up to 4, at least 4."""
+    return max(4, (nvals + 3) & ~3)
+
+
+def refuse_dense_overflow(count_overflow) -> None:
+    """Raise when a dense table reports ``[groups, overflow]`` with the overflow flag set: a key fell outside the
+    range the table was sized for, so some rows were not aggregated."""
+    if count_overflow[1]:
+        raise _lib.B200Error("dense group table saw a key outside its measured range")
+
+
 class GroupTable:
-    """Owner of one device hash table (mb200_gb_table)."""
+    """Owner of one device group table (mb200_gb_table): hashed (``GroupTable(capacity, nvals, flags)``) or dense
+    (``GroupTable.dense``; ``kbase`` is its first key, None for a hashed table)."""
+
+    kbase = None
 
     def __init__(self, group_capacity: int, nvals: int, flags: int):
         self.lib = _lib.load()
@@ -270,32 +289,42 @@ class GroupTable:
     @classmethod
     def dense(cls, key_min: int, key_max: int, nvals: int, flags: int):
         """Direct-addressed table for keys in [key_min, key_max] (mb200_gb_create_dense)."""
-        self = cls.__new__(cls)
-        self.lib = _lib.load()
-        self.handle = C.c_void_p()
-        self.capacity = R = int(key_max) - int(key_min) + 1
-        self.kbase = int(key_min)
-        self.nvals, self.flags = int(nvals), int(flags)
         # the arrays live in torch's allocator (layout: include/modin_b200.h) so that the multi-GPU
         # reduce can run NCCL collectives on them in place
         t = torch_mod()
         dev = current_device()
-        vs = max(4, (self.nvals + 3) & ~3)
-        has_acc = self.flags & (_lib.GB_SUM | _lib.GB_MIN | _lib.GB_MAX)
-        self.acc = t.empty(R * vs, dtype=t.float64 if self.flags & _lib.GB_SUM else t.int64, device=dev) if has_acc else None
-        self.cnt = t.empty(R * vs, dtype=t.int64, device=dev) if self.flags & _lib.GB_COUNT else None
-        self.size = t.empty(R, dtype=t.int64, device=dev) if self.flags & _lib.GB_SIZE else None
-        self.present = t.empty(4 * ((R + 3) // 4), dtype=t.uint8, device=dev)
-        ptr = lambda x: x.data_ptr() if x is not None else None  # noqa: E731
-        _lib.check(self.lib.mb200_gb_create_dense(C.byref(self.handle), int(key_min), int(key_max), self.nvals,
-                                                  self.flags, ptr(self.acc), ptr(self.cnt), ptr(self.size),
-                                                  ptr(self.present), current_stream()))  # fmt: skip
+        R, vs = int(key_max) - int(key_min) + 1, value_stride(nvals)
+        arrays = {}
+        if flags & _GB_ACC:
+            arrays["acc"] = t.empty(R * vs, dtype=t.float64 if flags & _lib.GB_SUM else t.int64, device=dev)
+        if flags & _lib.GB_COUNT:
+            arrays["cnt"] = t.empty(R * vs, dtype=t.int64, device=dev)
+        if flags & _lib.GB_SIZE:
+            arrays["size"] = t.empty(R, dtype=t.int64, device=dev)
+        arrays["present"] = t.empty(4 * ((R + 3) // 4), dtype=t.uint8, device=dev)
+        return cls._dense_table(int(key_min), R, nvals, flags, arrays)
+
+    @classmethod
+    def _dense_table(cls, kbase: int, nkeys: int, nvals: int, flags: int, arrays: dict, parent=None):
+        """A dense table over keys ``[kbase, kbase + nkeys)`` on the given arrays: a fresh one
+        (mb200_gb_create_dense) or, with ``parent``, a slice of it that inherits its overflow flag
+        (mb200_gb_adopt_dense)."""
+        self = cls.__new__(cls)
+        self.lib, self.handle = _lib.load(), C.c_void_p()
+        self.kbase, self.capacity, self.nvals, self.flags = kbase, nkeys, int(nvals), int(flags)
+        self.acc, self.cnt, self.size, self.present = (arrays.get(n) for n in _DENSE_ARRAYS)
+        ptrs = [x.data_ptr() if x is not None else None for x in (self.acc, self.cnt, self.size, self.present)]
+        args = (C.byref(self.handle), kbase, kbase + nkeys - 1, self.nvals, self.flags, *ptrs)
+        if parent is None:
+            _lib.check(self.lib.mb200_gb_create_dense(*args, current_stream()))
+        else:
+            _lib.check(self.lib.mb200_gb_adopt_dense(*args, parent.handle, current_stream()))
         return self
 
     def collective_arrays(self):
         """(tensor, reduce-op, elements per key) triples whose element-wise reduction over ranks merges dense tables."""
         acc_op = "sum" if self.flags & _lib.GB_SUM else ("min" if self.flags & _lib.GB_MIN else "max")
-        vs = max(4, (self.nvals + 3) & ~3)
+        vs = value_stride(self.nvals)
         out = [(self.acc, acc_op, vs), (self.cnt, "sum", vs), (self.size, "sum", 1), (self.present, "max", 1)]
         return [(x, op, per) for x, op, per in out if x is not None]
 
@@ -308,23 +337,12 @@ class GroupTable:
         t = torch_mod()
         if self.capacity % chunk or chunk % 4:
             raise ValueError("dense table is not padded to equal, 4-key-aligned chunks")
-        sl = GroupTable.__new__(GroupTable)
-        sl.lib, sl.handle = self.lib, C.c_void_p()
-        sl.capacity, sl.nvals, sl.flags = int(chunk), self.nvals, self.flags
-        sl.kbase = self.kbase + r * chunk
-        sl.acc = sl.cnt = sl.size = sl.present = None
-        for name, (x, op, per) in zip(self._array_names(), self.collective_arrays()):
-            out = t.empty(chunk * per, dtype=x.dtype, device=x.device)
-            reduce_scatter_fn(out, x[: self.capacity * per], op)
-            setattr(sl, name, out)
-        ptr = lambda x: x.data_ptr() if x is not None else None  # noqa: E731
-        _lib.check(self.lib.mb200_gb_adopt_dense(C.byref(sl.handle), sl.kbase, sl.kbase + chunk - 1, sl.nvals,
-                                                 sl.flags, ptr(sl.acc), ptr(sl.cnt), ptr(sl.size), ptr(sl.present),
-                                                 self.handle, current_stream()))  # fmt: skip
-        return sl
-
-    def _array_names(self):
-        return [n for n in ("acc", "cnt", "size", "present") if getattr(self, n) is not None]
+        names = [n for n in _DENSE_ARRAYS if getattr(self, n) is not None]
+        arrays = {}
+        for name, (x, op, per) in zip(names, self.collective_arrays()):
+            arrays[name] = t.empty(chunk * per, dtype=x.dtype, device=x.device)
+            reduce_scatter_fn(arrays[name], x[: self.capacity * per], op)
+        return self._dense_table(self.kbase + r * chunk, int(chunk), self.nvals, self.flags, arrays, parent=self)
 
     def window(self, gid_lo: int, gid_hi: int):
         _lib.check(self.lib.mb200_gb_dense_window(self.handle, int(gid_lo), int(gid_hi)))
@@ -357,12 +375,15 @@ class GroupTable:
         _lib.check(self.lib.mb200_gb_ngroups(self.handle, C.byref(ng), C.byref(ov), current_stream()))
         return int(ng.value), bool(ov.value)
 
+    def _outputs(self, rows: int):
+        """Empty (keys, sums, cnts, sizes) columns of ``rows`` rows for what this table emits."""
+        sums = [DeviceColumn.empty(rows, np.float64) for _ in range(self.nvals)] if self.flags & _GB_ACC else None
+        cnts = [DeviceColumn.empty(rows, np.int64) for _ in range(self.nvals)] if self.flags & _lib.GB_COUNT else None
+        sizes = DeviceColumn.empty(rows, np.int64) if self.flags & _lib.GB_SIZE else None
+        return DeviceColumn.empty(rows, np.int64), sums, cnts, sizes
+
     def emit(self, ngroups: int, sort: bool = True):
-        keys = DeviceColumn.empty(ngroups, np.int64)
-        has_acc = self.flags & (_lib.GB_SUM | _lib.GB_MIN | _lib.GB_MAX)
-        sums = [DeviceColumn.empty(ngroups, np.float64) for _ in range(self.nvals)] if has_acc else None
-        cnts = [DeviceColumn.empty(ngroups, np.int64) for _ in range(self.nvals)] if self.flags & _lib.GB_COUNT else None
-        sizes = DeviceColumn.empty(ngroups, np.int64) if self.flags & _lib.GB_SIZE else None
+        keys, sums, cnts, sizes = self._outputs(ngroups)
         scratch = _scratch(self.lib.mb200_gb_emit_scratch_bytes(ngroups), "gb_emit")
         _lib.check(
             self.lib.mb200_gb_emit(
@@ -377,15 +398,11 @@ class GroupTable:
     def emit_async(self):
         """Dense tables: emit WITHOUT asking the device how many groups there are -- the outputs have room for every
         key of the table's range, the count is left in a device int64[2] ``{groups, overflow}``
-        (``mb200_gb_emit_dense_async``).  Returns ``(keys, sums, cnts, sizes, count_dev)``; the columns are valid up
-        to ``count_dev[0]``."""
+        (``mb200_gb_emit_dense_async``; ``refuse_dense_overflow`` checks it once read).  Returns
+        ``(keys, sums, cnts, sizes, count_dev)``; the columns are valid up to ``count_dev[0]``."""
         t = torch_mod()
         cap = self.capacity
-        keys = DeviceColumn.empty(cap, np.int64)
-        has_acc = self.flags & (_lib.GB_SUM | _lib.GB_MIN | _lib.GB_MAX)
-        sums = [DeviceColumn.empty(cap, np.float64) for _ in range(self.nvals)] if has_acc else None
-        cnts = [DeviceColumn.empty(cap, np.int64) for _ in range(self.nvals)] if self.flags & _lib.GB_COUNT else None
-        sizes = DeviceColumn.empty(cap, np.int64) if self.flags & _lib.GB_SIZE else None
+        keys, sums, cnts, sizes = self._outputs(cap)
         count = t.empty(2, dtype=t.int64, device=current_device())
         scratch = _scratch(self.lib.mb200_gb_emit_scratch_bytes(cap), "gb_emit")
         _lib.check(
@@ -408,6 +425,29 @@ class GroupTable:
             self.close()
         except Exception:
             pass
+
+
+# The table driver works through the table's library calls only (accumulate / merge_partial / ngroups / emit), so that
+# whatever stands in for a table needs nothing else.
+def fill_table(table, items, partial: bool = False):
+    """Aggregate every input into ``table``: raw ``(keys, vals)`` rows (``accumulate``), or with ``partial`` the
+    emitted ``(keys, sums, cnts, sizes)`` of other tables (``merge_partial``).  Returns the table."""
+    for item in items:
+        if partial:
+            table.merge_partial(*item)
+        else:
+            table.accumulate(item[0], item[1])
+    return table
+
+
+def emit_counted(table, sort: bool = True):
+    """Count the groups of ``table`` (one host round trip) and emit them: ``(keys, sums, cnts, sizes)``, or None when
+    a hashed table overflowed (recreate it larger).  A dense table that saw a key outside its range is refused."""
+    ng, overflow = table.ngroups()
+    if overflow and table.kbase is None:
+        return None
+    refuse_dense_overflow((ng, overflow))
+    return table.emit(ng, sort=sort)
 
 
 DENSE_TABLE_MAX_BYTES = 8 << 30
@@ -480,17 +520,83 @@ def dense_range_ok(lo: int, hi: int, cap: int, total_rows: int, nvals: int, flag
     rng = hi - lo + 1
     if rng > (1 << 29) or rng > max(4 * cap, total_rows // 2, 1 << 16):
         return False
-    vstride = max(4, (nvals + 3) & ~3)
-    arrays = (1 if flags & (_lib.GB_SUM | _lib.GB_MIN | _lib.GB_MAX) else 0) + (1 if flags & _lib.GB_COUNT else 0)
-    return rng * (vstride * 8 * arrays + 9) <= DENSE_TABLE_MAX_BYTES
+    arrays = (1 if flags & _GB_ACC else 0) + (1 if flags & _lib.GB_COUNT else 0)
+    return rng * (value_stride(nvals) * 8 * arrays + 9) <= DENSE_TABLE_MAX_BYTES
+
+
+def _job_key_range(key_cols: Sequence[DeviceColumn], lo: int, hi: int, rows: int):
+    """Job-wide ``(min, max, rows)`` of key columns whose rows are sharded over the ranks, from this rank's.  Every
+    rank must size its table alike, so the ranks agree ONCE per set of key columns (one small all_gather + one D2H)
+    and the answer is remembered on the first of them -- columns are immutable and so is the job."""
+    from . import dist
+
+    if not dist.is_distributed():
+        return lo, hi, rows
+    sig = (dist.world_size(), tuple(id(k.data) for k in key_cols))
+    anchor = key_cols[0].stats
+    if anchor.job is None or anchor.job[0] != sig:
+        t = torch_mod()
+        trip = dist.all_gather_small(t.tensor([lo, hi, rows], dtype=t.int64, device=current_device()))
+        anchor.job = (sig, (min(r[0] for r in trip), max(r[1] for r in trip), sum(r[2] for r in trip)))
+    return anchor.job[1]
+
+
+class TablePlan(NamedTuple):
+    """The group table a groupby fills (``plan_table``)."""
+
+    nvals: int
+    flags: int
+    dense: Optional[tuple]  # (first key, last key) of a dense table; None: a hash table
+    capacity: int  # groups a hash table starts with
+    rows: int  # rows to aggregate: a hash table never needs more groups than that
+    skewed: bool  # accumulate with the hot-group cache
+    chunk: int = 0  # job-wide dense table over several ranks: keys per rank (the range is padded to ranks * chunk)
+
+    def create(self, capacity: Optional[int] = None) -> GroupTable:
+        if self.dense is not None:
+            table = GroupTable.dense(self.dense[0], self.dense[1], self.nvals, self.flags)
+        else:
+            table = GroupTable(self.capacity if capacity is None else capacity, self.nvals, self.flags)
+        table.hint_skew(self.skewed)
+        return table
+
+
+def plan_table(key_cols: Sequence[DeviceColumn], nvals: int, flags: int, capacity_hint: int, partial: bool = False,
+               job_wide: bool = False) -> Optional[TablePlan]:
+    """Dense or hashed: a dense (direct-addressed) table over the keys' range when ``GroupbyDenseKeys`` is on and
+    ``dense_range_ok`` accepts the range for ``max(1024, min(capacity_hint, rows))`` expected groups, else a hash
+    table of that many groups.  The hot-group cache is hinted from the keys' sample, except for partial tables.
+
+    ``job_wide``: the key columns are this rank's part of a job that fills ONE dense table per rank and merges them
+    across ranks.  Range and row count are then the job's (``_job_key_range``), the table spans the range padded to
+    one equal chunk per rank, and the answer is None when no dense table fits."""
+    from .config import GroupbyDenseKeys
+
+    dense_keys = GroupbyDenseKeys.get()
+    if job_wide and not dense_keys:
+        return None
+    lo, hi, sampled, dup = key_stats(key_cols)  # column metadata: no pass over the keys, no sync, once known
+    rows = sum(len(k) for k in key_cols)
+    if job_wide:
+        lo, hi, rows = _job_key_range(key_cols, lo, hi, rows)  # `sampled` / `dup` stay local, like the cache
+    cap = max(1024, min(int(capacity_hint), rows))
+    dense = (lo, hi) if dense_keys and lo <= hi and dense_range_ok(lo, hi, cap, rows, nvals, flags) else None
+    chunk = 0
+    if job_wide:
+        from . import dist
+
+        if dense is None:
+            return None
+        if dist.is_distributed() and dist.world_size() > 1:
+            chunk = dist.dense_chunk(hi - lo + 1, dist.world_size())
+            dense = (lo, lo + dist.world_size() * chunk - 1)
+    return TablePlan(nvals, flags, dense, cap, rows, not partial and keys_are_skewed(sampled, dup), chunk)
 
 
 def hash_aggregate(key_cols_vals, flags: int, capacity_hint: int, partial: bool = False, sort: bool = True):
     """Aggregate a list of (keys, vals[, cnts, sizes]) inputs into one table and emit it: a dense
     (direct-addressed) table when the key range allows, else the hash table, grown when it
     overflows.  Returns (keys, sums, cnts, sizes) device columns."""
-    from .config import GroupbyDenseKeys
-
     nvals = len(key_cols_vals[0][1]) if key_cols_vals[0][1] else 0
     if nvals > _lib.MAX_COLS:
         # a table holds at most MAX_COLS value columns: aggregate them MAX_COLS at a time.  Every pass sees the same
@@ -502,47 +608,19 @@ def hash_aggregate(key_cols_vals, flags: int, capacity_hint: int, partial: bool 
             parts.append(hash_aggregate(items, flags, capacity_hint, partial=partial, sort=True))
         join = lambda cols: [c for cs in cols for c in cs] if cols[0] is not None else None  # noqa: E731
         return parts[0][0], join([p[1] for p in parts]), join([p[2] for p in parts]), parts[0][3]
-    cap = max(int(capacity_hint), 1024)
-    total_rows = sum(len(item[0]) for item in key_cols_vals)
-    skewed = False
-    if total_rows > 0:
-        # key statistics are column metadata (KeyStats): free once known, one pass for a column of unknown origin
-        lo, hi, sampled, dup = key_stats([item[0] for item in key_cols_vals])
-        kr = None if lo > hi else (lo, hi)
-        skewed = not partial and keys_are_skewed(sampled, dup)
-        if GroupbyDenseKeys.get() and kr is not None and dense_range_ok(kr[0], kr[1], cap, total_rows, nvals, flags):
-            table = GroupTable.dense(kr[0], kr[1], nvals, flags)
-            table.hint_skew(skewed)
-            try:
-                for item in key_cols_vals:
-                    if partial:
-                        table.merge_partial(*item)
-                    else:
-                        table.accumulate(item[0], item[1])
-                ng, overflow = table.ngroups()
-                if overflow:
-                    raise _lib.B200Error("dense group table saw a key outside its measured range")
-                return table.emit(ng, sort=False)
-            finally:
-                table.close()
+    plan = plan_table([item[0] for item in key_cols_vals], nvals, flags, capacity_hint, partial=partial)
+    cap = plan.capacity
     while True:
-        table = GroupTable(cap, nvals, flags)
-        table.hint_skew(skewed)
+        table = plan.create(cap)
         try:
-            for item in key_cols_vals:
-                if partial:
-                    table.merge_partial(*item)
-                else:
-                    table.accumulate(item[0], item[1])
-            ng, overflow = table.ngroups()
-            if not overflow:
-                return table.emit(ng, sort=sort)
+            out = emit_counted(fill_table(table, key_cols_vals, partial), sort=sort)
         finally:
             table.close()
-        total_rows = sum(len(item[0]) for item in key_cols_vals)
-        if cap >= max(total_rows, 1024):
+        if out is not None:
+            return out
+        if cap >= max(plan.rows, 1024):
             raise _lib.B200Error("group table overflow even with capacity == number of rows")
-        cap = min(max(cap * 4, 1024), max(total_rows, 1024))
+        cap = min(max(cap * 4, 1024), max(plan.rows, 1024))
 
 
 # ------------------------------------------------------------------ broadcast hash join

@@ -477,16 +477,13 @@ class B200AxisPartition:
     def deploy_axis_func(cls, axis, func, f_args, f_kwargs, num_splits, maintain_partitioning, blocks,
                          lengths=None, manual_partition=False, min_block_size=None):  # fmt: skip
         """axpart.py:396-499: concat the blocks along ``axis``, run ``func`` once, split the result.
-        A device functor that declares collective hooks is run as  pre -> collective -> post  when
-        the job spans several ranks (the other ranks hold the remaining blocks of this axis)."""
+        When the job spans several ranks (the other ranks hold the remaining blocks of this axis), a reduce-phase
+        device functor finishes with its own collective (``functors._spans_ranks``)."""
         gathered = concat_rows(blocks) if axis == 0 else concat_cols(blocks)
         fn, bargs, bkw = unwrap(func)
         args = tuple(bargs) + tuple(f_args or ())
         kwargs = {**bkw, **(f_kwargs or {})}
-        if dist.is_distributed() and axis == 0 and hasattr(fn, "run_distributed") and not gathered.replicated:
-            result = fn.run_distributed(gathered, *args, **kwargs)
-        else:
-            result = _inherit_replicated(fn(gathered, *args, **kwargs), (gathered, *args))
+        result = _inherit_replicated(fn(gathered, *args, **kwargs), (gathered, *args))
         if manual_partition:
             lengths_ = lengths
         elif num_splits == 1:

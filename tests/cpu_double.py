@@ -119,39 +119,6 @@ def reduce_columns(op, cols, skipna=True, variant=0, centers=None):
     return vals, cnts
 
 
-def hash_aggregate(items, flags, capacity_hint, partial=False, sort=True):
-    keys = np.concatenate([_np(it[0]) for it in items])
-    nv = len(items[0][1]) if items[0][1] else 0
-    df = pandas.DataFrame({"k": keys})
-    uniq = np.sort(np.unique(keys))
-    g = df.groupby("k", sort=True)
-    sums = cnts = sizes = None
-    if flags & _lib.GB_SUM:
-        sums = []
-        for v in range(nv):
-            x = np.concatenate([_np(it[1][v]) for it in items])
-            sums.append(_col(pandas.Series(np.where(np.isnan(x), 0.0, x)).groupby(keys, sort=True).sum().to_numpy()))
-    for flag, fn in ((_lib.GB_MIN, "min"), (_lib.GB_MAX, "max")):
-        if flags & flag:
-            sums = []
-            for v in range(nv):
-                x = np.concatenate([_np(it[1][v]) for it in items])
-                sums.append(_col(getattr(pandas.Series(x).groupby(keys, sort=True), fn)().to_numpy().astype(np.float64)))
-    if flags & _lib.GB_COUNT:
-        cnts = []
-        for v in range(nv):
-            if partial:
-                c = np.concatenate([_np(it[2][v]) for it in items])
-            else:
-                c = (~np.isnan(np.concatenate([_np(it[1][v]) for it in items]))).astype(np.int64)
-            cnts.append(_col(pandas.Series(c).groupby(keys, sort=True).sum().to_numpy().astype(np.int64)))
-    if flags & _lib.GB_SIZE:
-        z = np.concatenate([_np(it[3]) for it in items]) if partial else np.ones(len(keys), dtype=np.int64)
-        sizes = _col(pandas.Series(z).groupby(keys, sort=True).sum().to_numpy().astype(np.int64))
-    del g
-    return _col(uniq.astype(np.int64)), sums, cnts, sizes
-
-
 def key_range_device(key_cols):
     ks = [_np(k) for k in key_cols if len(k)]
     if not ks:
@@ -159,44 +126,88 @@ def key_range_device(key_cols):
     return torch.tensor([min(int(k.min()) for k in ks), max(int(k.max()) for k in ks), 0, 0], dtype=torch.int64)
 
 
-class GroupTable:
-    """numpy stand-in for the DENSE device table (same array layout as include/modin_b200.h), so that the
-    fused map+reduce path and its cross-rank merge by collectives run under gloo."""
+class GroupTable(ops.GroupTable):
+    """numpy stand-in for the device group table, hashed or dense (dense arrays in the layout of include/modin_b200.h,
+    so that the fused path's cross-rank merge by collectives runs under gloo).  Only the calls into the library are
+    replaced: filling, the counted emit, the dense-or-hashed choice and the reduce-scatter are the real code.
+
+    ``created`` lists the kind of every table made ("hashed", "dense", or "slice" for a reduce-scattered part);
+    ``round_trips`` counts ``ngroups()`` calls, the host round trip of a counted emit."""
+
+    created: list = []
+    round_trips = 0
+
+    def __init__(self, group_capacity, nvals, flags):
+        R, vs = int(group_capacity), ops.value_stride(nvals)
+        arrays = {"acc": torch.empty(R * vs, dtype=torch.float64 if flags & _lib.GB_SUM else torch.int64),
+                  "cnt": torch.empty(R * vs, dtype=torch.int64), "size": torch.empty(R, dtype=torch.int64)}  # fmt: skip
+        self._setup(None, R, nvals, flags, arrays, "hashed")
+        self.keys = np.zeros(0, dtype=np.int64)  # distinct keys, by group id
 
     @classmethod
-    def dense(cls, key_min, key_max, nvals, flags):
-        self = cls()
-        self.kbase, self.R, self.nvals, self.flags = int(key_min), int(key_max) - int(key_min) + 1, nvals, flags
-        self.vs = max(4, (nvals + 3) & ~3)
-        R, vs = self.R, self.vs
-        self.acc = self.cnt = self.size = None
-        if flags & _lib.GB_SUM:
-            self.acc = torch.zeros(R * vs, dtype=torch.float64)
-        elif flags & _lib.GB_MIN:
-            self.acc = torch.full((R * vs,), np.iinfo(np.int64).max, dtype=torch.int64)
-        elif flags & _lib.GB_MAX:
-            self.acc = torch.full((R * vs,), np.iinfo(np.int64).min, dtype=torch.int64)
-        if flags & _lib.GB_COUNT:
-            self.cnt = torch.zeros(R * vs, dtype=torch.int64)
-        if flags & _lib.GB_SIZE:
-            self.size = torch.zeros(R, dtype=torch.int64)
-        self.present = torch.zeros(4 * ((R + 3) // 4), dtype=torch.uint8)
-        self.win = (0, R)
+    def _dense_table(cls, kbase, nkeys, nvals, flags, arrays, parent=None):
+        self = cls.__new__(cls)
+        self._setup(kbase, nkeys, nvals, flags, arrays, "dense" if parent is None else "slice")
+        if parent is not None:  # the reduce-scattered arrays hold merged values
+            self.overflow = parent.overflow
         return self
+
+    def _setup(self, kbase, capacity, nvals, flags, arrays, kind):
+        self.kbase, self.capacity, self.nvals, self.flags = kbase, int(capacity), int(nvals), int(flags)
+        self.vs = ops.value_stride(nvals)
+        self.acc, self.cnt, self.size, self.present = (arrays.get(n) for n in ("acc", "cnt", "size", "present"))
+        if not flags & (_lib.GB_SUM | _lib.GB_MIN | _lib.GB_MAX):
+            self.acc = None
+        if not flags & _lib.GB_COUNT:
+            self.cnt = None
+        if not flags & _lib.GB_SIZE:
+            self.size = None
+        if kind != "slice":  # what mb200_gb_create / _create_dense clear the arrays to
+            if self.acc is not None:
+                ident = 0 if flags & _lib.GB_SUM else np.iinfo(np.int64).max if flags & _lib.GB_MIN else np.iinfo(np.int64).min
+                self.acc.fill_(ident)
+            for x in (self.cnt, self.size, self.present):
+                if x is not None:
+                    x.zero_()
+        self.overflow = False
+        self.win = (0, self.capacity)
+        GroupTable.created.append(kind)
 
     @staticmethod
     def _ordered(x):  # order-preserving int64 image of float64 (csrc/groupby.cu f64_to_ordered)
         b = x.view(np.int64)
         return b ^ ((b >> 63) & np.int64(0x7FFFFFFFFFFFFFFF))
 
-    def accumulate(self, keys, vals):
-        g = _np(keys) - self.kbase
-        assert len(g) == 0 or (g.min() >= 0 and g.max() < self.R)
-        self.present.numpy()[g] = 1
+    def _gids(self, keys):
+        """Group id of every row; ``capacity`` for a row whose key found no room (the table then overflows)."""
+        k = _np(keys)
+        if self.kbase is not None:
+            g = k - self.kbase
+            outside = (g < 0) | (g >= self.capacity)
+            self.overflow |= bool(outside.any())
+            return np.where(outside, self.capacity, g)
+        new = np.setdiff1d(k, self.keys)
+        room = self.capacity - len(self.keys)
+        if len(new) > room:
+            self.overflow = True
+        self.keys = np.concatenate([self.keys, new[:room]])
+        order = np.argsort(self.keys, kind="stable")
+        pos = np.minimum(np.searchsorted(self.keys[order], k), max(len(order) - 1, 0))
+        found = self.keys[order][pos] == k if len(order) else np.zeros(len(k), dtype=bool)
+        return np.where(found, order[pos] if len(order) else 0, self.capacity)
+
+    def _add(self, keys, vals, cnts=None, sizes=None):
+        """Rows into the table: raw values (count the non-NaN ones, one row each), or with ``cnts`` / ``sizes`` the
+        columns of partial tables.  NaN values are skipped either way, as the kernel does."""
+        g = self._gids(keys)
+        live = g < self.capacity
+        g = g[live]
+        if self.present is not None:
+            self.present.numpy()[g] = 1
         if self.size is not None:
-            np.add.at(self.size.numpy(), g, 1)
-        for v, col in enumerate(vals):
-            x = _np(col)
+            np.add.at(self.size.numpy(), g, _np(sizes)[live] if sizes is not None else 1)
+        for v, col in enumerate(vals or []):
+            x = _np(col)[live]
             ok = ~np.isnan(x)
             o = g[ok] * self.vs + v
             if self.flags & _lib.GB_SUM:
@@ -206,60 +217,60 @@ class GroupTable:
             elif self.flags & _lib.GB_MAX:
                 np.maximum.at(self.acc.numpy(), o, self._ordered(x[ok]))
             if self.cnt is not None:
-                np.add.at(self.cnt.numpy(), o, 1)
+                np.add.at(self.cnt.numpy(), g * self.vs + v, _np(cnts[v])[live] if cnts is not None else ok.astype(np.int64))
 
-    def collective_arrays(self):
-        acc_op = "sum" if self.flags & _lib.GB_SUM else ("min" if self.flags & _lib.GB_MIN else "max")
-        out = [(self.acc, acc_op, self.vs), (self.cnt, "sum", self.vs), (self.size, "sum", 1), (self.present, "max", 1)]
-        return [(x, op, per) for x, op, per in out if x is not None]
+    def accumulate(self, keys, vals):
+        self._add(keys, vals)
 
-    def reduce_scatter(self, chunk, reduce_scatter_fn, r):
-        assert self.R % chunk == 0 and chunk % 4 == 0
-        sl = GroupTable()
-        sl.kbase, sl.R, sl.nvals, sl.flags, sl.vs = self.kbase + r * chunk, chunk, self.nvals, self.flags, self.vs
-        sl.acc = sl.cnt = sl.size = None
-        sl.win = (0, chunk)
-        names = [n for n in ("acc", "cnt", "size", "present") if getattr(self, n) is not None]
-        for name, (x, op, per) in zip(names, self.collective_arrays()):
-            out = torch.empty(chunk * per, dtype=x.dtype)
-            reduce_scatter_fn(out, x[: self.R * per], op)
-            setattr(sl, name, out)
-        return sl
+    def merge_partial(self, keys, sums, cnts=None, sizes=None):
+        self._add(keys, sums, cnts, sizes)
 
     def hint_skew(self, skewed):
         pass
 
     def window(self, lo, hi):
-        assert lo % 4 == 0 and (hi % 4 == 0 or hi == self.R) and 0 <= lo <= hi <= self.R
+        assert lo % 4 == 0 and (hi % 4 == 0 or hi == self.capacity) and 0 <= lo <= hi <= self.capacity
         self.win = (int(lo), int(hi))
 
-    def _gids(self):
-        lo, hi = self.win
-        return lo + np.nonzero(self.present.numpy()[lo:hi])[0]
+    def _rows(self, sort):
+        """Group ids in emit order: a dense table's present keys of the window, ascending; a hashed table's groups,
+        ascending by key when ``sort``."""
+        if self.kbase is not None:
+            lo, hi = self.win
+            return lo + np.nonzero(self.present.numpy()[lo:hi])[0]
+        g = np.arange(min(len(self.keys), self.capacity))
+        return g[np.argsort(self.keys[g], kind="stable")] if sort else g
 
     def ngroups(self):
-        return len(self._gids()), False
+        GroupTable.round_trips += 1
+        return len(self._rows(False)), self.overflow
 
-    def emit(self, ngroups, sort=True):
-        g = self._gids()
-        assert len(g) == ngroups
+    def _emit(self, g):
         sums = cnts = sizes = None
         if self.acc is not None:
-            a = self.acc.numpy().reshape(self.R, self.vs)[g]
+            a = self.acc.numpy().reshape(self.capacity, self.vs)[g]
             if not self.flags & _lib.GB_SUM:
                 empty = a == (np.iinfo(np.int64).max if self.flags & _lib.GB_MIN else np.iinfo(np.int64).min)
                 a = np.where(empty, np.nan, (a ^ ((a >> 63) & np.int64(0x7FFFFFFFFFFFFFFF))).view(np.float64))
             sums = [_col(np.ascontiguousarray(a[:, v])) for v in range(self.nvals)]
         if self.cnt is not None:
-            c = self.cnt.numpy().reshape(self.R, self.vs)[g]
+            c = self.cnt.numpy().reshape(self.capacity, self.vs)[g]
             cnts = [_col(np.ascontiguousarray(c[:, v])) for v in range(self.nvals)]
         if self.size is not None:
             sizes = _col(self.size.numpy()[g])
-        return _col((g + self.kbase).astype(np.int64)), sums, cnts, sizes
+        keys = g + self.kbase if self.kbase is not None else self.keys[g]
+        return _col(keys.astype(np.int64)), sums, cnts, sizes
+
+    def emit(self, ngroups, sort=True):
+        if self.overflow and self.kbase is None:
+            raise _lib.B200Error("mb200_gb_emit: table overflowed: recreate with a larger group capacity")
+        g = self._rows(sort)
+        assert len(g) == ngroups
+        return self._emit(g)
 
     def emit_async(self):
-        ng, _ = self.ngroups()
-        keys, sums, cnts, sizes = self.emit(ng, sort=False)
+        g = self._rows(False)
+        keys, sums, cnts, sizes = self._emit(g)
         lo, hi = self.win
         cap = hi - lo
 
@@ -270,7 +281,7 @@ class GroupTable:
             return _col(np.concatenate([a, np.zeros(cap - len(a), dtype=a.dtype)]))
 
         return (pad(keys), [pad(c) for c in sums] if sums else None, [pad(c) for c in cnts] if cnts else None, pad(sizes),
-                torch.tensor([ng, 0], dtype=torch.int64))
+                torch.tensor([len(g), int(self.overflow)], dtype=torch.int64))
 
     def close(self):
         pass
@@ -466,7 +477,7 @@ def installed():
 
     saved = {
         "current_device": block.current_device,
-        **{n: getattr(ops, n) for n in ("map_columns", "reduce_columns", "hash_aggregate", "JoinTable", "take_columns",
+        **{n: getattr(ops, n) for n in ("map_columns", "reduce_columns", "JoinTable", "take_columns",
                                         "compact_hits", "cast_columns_f64", "cast_columns_i64", "gen_f64", "gen_i64", "GroupTable",
                                         "key_range_device", "sort_pairs", "iota", "full_column", "expand_matches", "digitize", "run_starts", "concat_columns", "cum_partials", "cum_carry", "cum_apply")},
     }  # fmt: skip
@@ -477,7 +488,7 @@ def installed():
     ops.cast_columns_i64 = cast_columns_i64
     block.current_device = lambda: torch.device("cpu")
     ops.current_device = block.current_device
-    ops.map_columns, ops.reduce_columns, ops.hash_aggregate = map_columns, reduce_columns, hash_aggregate
+    ops.map_columns, ops.reduce_columns = map_columns, reduce_columns
     ops.JoinTable, ops.take_columns, ops.compact_hits, ops.cast_columns_f64 = JoinTable, take_columns, compact_hits, \
         cast_columns_f64  # fmt: skip
     ops.gen_f64 = lambda n, seed, col, row_offset=0, nan_per_64k=0: _col(synth.gen_f64(n, seed, col, row_offset, nan_per_64k))
