@@ -1,14 +1,15 @@
-"""Operator templates: Map, TreeReduce, Binary, GroupByReduce.
+"""Operator templates: Map, TreeReduce, Reduce, Fold, Binary.
 
 Same contract as modin/core/dataframe/algebra/: ``Template.register(func, ...)`` returns a
 ``caller(query_compiler, *args, **kwargs) -> query_compiler`` closure that calls the matching
 core-dataframe method (``map`` / ``tree_reduce`` / ``n_ary_op`` / ``broadcast_apply`` /
-``groupby_reduce``).  The registered ``func`` is a device functor (functors.py) with the pandas
+``reduce`` / ``fold``).  The registered ``func`` is a device functor (functors.py) with the pandas
 method's calling convention; arguments are bound with ``Bound`` (the inspectable twin of the
 reference's ``lambda x: function(x, *args, **kwargs)``) so the partition call queue can fuse.
 
-Reference: operator.py:21-64, map.py:32-70, tree_reduce.py:33-82, binary.py:296-460,
-groupby.py:55-102, 303-450, 687-790.
+Reference: operator.py:21-64, map.py:32-70, tree_reduce.py:33-82, reduce.py:32-71, fold.py:32-95,
+binary.py:296-460.  The groupby aggregations are not a template here: ``query_compiler.device_operations`` calls
+``groupby_reduce`` with the device functors directly, under both front doors.
 """
 
 from __future__ import annotations
@@ -169,40 +170,3 @@ class Binary(Operator):
 
         return caller
 
-
-class GroupByReduce(Operator):
-    """alg/groupby.py:33-790 restricted to what has a device implementation: ``by`` is a
-    one-column query compiler (``df.groupby("key")`` resolves the label to it in the API layer),
-    axis=0, as_index=True, sort=True, dropna irrelevant for int64 keys."""
-
-    @classmethod
-    def register(cls, map_func, reduce_func=None, **call_kwds):
-        if reduce_func is None:
-            reduce_func = map_func
-
-        def build_groupby_reduce_method(query_compiler, by, axis, groupby_kwargs, agg_args, agg_kwargs, drop=False,
-                                        **kwargs):  # fmt: skip
-            return cls.caller(query_compiler, by, map_func, reduce_func, axis, groupby_kwargs, agg_args, agg_kwargs,
-                              drop=drop, **call_kwds, **kwargs)  # fmt: skip
-
-        return build_groupby_reduce_method
-
-    @classmethod
-    def caller(cls, query_compiler, by, map_func, reduce_func, axis, groupby_kwargs, agg_args, agg_kwargs,
-               drop=False, method=None, default_to_pandas_func=None, finalizer_fn=None):  # fmt: skip
-        if axis != 0:
-            raise NotImplementedError("groupby along axis=1 defaults to pandas in the reference; not on the B200 path")
-        if not isinstance(by, type(query_compiler)):
-            raise NotImplementedError("`by` must resolve to a column of a frame on the B200 path")
-        for key, allowed in (("as_index", (True, False)), ("level", (None,)), ("observed", (True, False, None))):
-            if groupby_kwargs.get(key, allowed[0]) not in allowed:
-                raise NotImplementedError(f"groupby({key}={groupby_kwargs[key]!r}) is not on the B200 path")
-        # alg/groupby.py:403-416: keys are sorted anyway
-        map_fn = Bound(map_func, agg_args, agg_kwargs)
-        reduce_fn = Bound(reduce_func, agg_args, agg_kwargs)
-        new_modin_frame = query_compiler._modin_frame.groupby_reduce(axis, by._modin_frame, map_fn, reduce_fn)
-        if not groupby_kwargs.get("as_index", True):
-            from .query_compiler import group_keys_to_columns
-
-            new_modin_frame = group_keys_to_columns(new_modin_frame)  # alg/groupby.py:278-294
-        return query_compiler.__constructor__(new_modin_frame)

@@ -111,17 +111,20 @@ def key_image(key_blocks: List[DeviceBlock]):
 
     One int64 key: the blocks themselves and ``None`` -- nothing is launched or allocated.  One float64 key: its
     order-preserving image under the key's own label (``float_image``) and ``FLOAT_KEY``.  Several int64 keys: their
-    packed image labelled ``PACKED_KEY`` and ``(packing plan, key labels)``."""
+    packed image labelled ``PACKED_KEY`` and ``(packing plan, key labels)``.  An image block keeps the row labels of
+    its key block, so it still lines up with the frame it groups."""
     first = key_blocks[0]
     if len(first.cols) > 1:
         plan = packing_plan(key_blocks)
-        label = pandas.Index([PACKED_KEY])
-        images = [DeviceBlock([pack(b, plan)], label, nrows=b.nrows, range_start=b.range_start) for b in key_blocks]
-        return images, (plan, list(first.columns))
+        return [_image_block(b, pack(b, plan), [PACKED_KEY]) for b in key_blocks], (plan, list(first.columns))
     if first.cols[0].dtype == np.float64:
-        return [DeviceBlock([float_image(b.cols[0])], b.columns, nrows=b.nrows, range_start=b.range_start)
-                for b in key_blocks], FLOAT_KEY  # fmt: skip
+        return [_image_block(b, float_image(b.cols[0]), b.columns) for b in key_blocks], FLOAT_KEY
     return key_blocks, None
+
+
+def _image_block(b: DeviceBlock, image: DeviceColumn, label) -> DeviceBlock:
+    return DeviceBlock([image], pandas.Index(label), nrows=b.nrows, range_start=b.range_start, index_cols=b.index_cols,
+                       index_names=b.index_names, index_host=b.index_host)  # fmt: skip
 
 
 def restore_keys(blocks: List[DeviceBlock], image, dropna: bool = True, names=None) -> List[DeviceBlock]:

@@ -93,7 +93,7 @@ def register(shims: bool | None = None):
 
     import modin.config as cfg
     from modin.config.envvars import Execution
-    from modin.core.dataframe.algebra import Binary, Fold, GroupByReduce, Map, Reduce, TreeReduce
+    from modin.core.dataframe import algebra as malg
     from modin.core.dataframe.pandas.dataframe.dataframe import PandasDataframe
     from modin.core.dataframe.pandas.partitioning.partition_manager import PandasDataframePartitionManager
     from modin.core.execution.dispatching.factories import factories
@@ -102,10 +102,9 @@ def register(shims: bool | None = None):
 
     from . import dist as bdist
     from . import functors as fx
-    from . import groupkeys as gk
     from . import partitioning as bp
     from .block import DeviceBlock, concat_cols
-    from .query_compiler import _dtypes_sum
+    from .query_compiler import _reset_row_index, device_operations
 
     # ---------------------------------------------------------------- partition manager
     class B200OnModinPartitionManager(bp.B200PartitionManager, PandasDataframePartitionManager):
@@ -351,65 +350,31 @@ def register(shims: bool | None = None):
                                frame.row_lengths, [1])  # fmt: skip
         return query_compiler.__constructor__(by_frame), name
 
-    # ---------------------------------------------------------------- GroupByReduce over device blocks
-    class B200GroupByReduce(GroupByReduce):
-        """alg/groupby.py: same template, but the per-block map / reduce bodies are the device functors
-        instead of ``df.groupby(...)`` on pandas blocks (alg/groupby.py:124-300)."""
+    def _by_level(groupby_agg):
+        """A groupby aggregation of ``device_operations`` that also takes ``groupby(level=0)``: the row labels are the
+        key (alg/groupby.py:355-390 hands ``level`` to pandas per block).  They already sit on the device (an index
+        column) or are a range (materialised with mb200_iota); the frame of one key column built from them goes down
+        the ordinary path, and the result's keys take the index level's own name."""
 
-        @classmethod
-        def register_agg(cls, agg: str):
-            map_f, red_f = fx.DevGroupbyMap(agg), fx.DevGroupbyReduce(agg)
-
-            def caller(query_compiler, by, axis, groupby_kwargs, agg_args, agg_kwargs, drop=False, **kwargs):
-                level = groupby_kwargs.get("level")
-                level_name = None
-                if by is None and level is not None and axis == 0:
-                    # groupby(level=0): the row labels are the key (alg/groupby.py:355-390 hands ``level`` to pandas per
-                    # block).  They already sit on the device (an index column) or are a range (materialised with
-                    # mb200_iota); the frame of one key column built from them goes down the ordinary path
-                    by, level_name = _labels_as_by(query_compiler, level)
-                elif level is not None:
+        def caller(query_compiler, by, axis, groupby_kwargs, agg_args, agg_kwargs, drop=False, **kwargs):
+            level = groupby_kwargs.get("level")
+            key_names = None
+            if level is not None:
+                if by is not None or axis != 0:
                     raise NotImplementedError("device groupby: `level=` together with `by` is not on the B200 path")
-                if axis != 0 or not isinstance(by, type(query_compiler)) or len(by.columns) < 1:
-                    raise NotImplementedError("device groupby: key columns of the same frame, axis=0")
-                frame, by_frame = query_compiler._modin_frame, by._modin_frame
-                # a float64 key or several int64 keys: the single-key groupby runs on their int64 image and the G
-                # result keys are restored afterwards (groupkeys.py); one int64 key is its own image
-                keys = [concat_cols([p.get() for p in row]) if len(row) > 1 else row[0].get() for row in by_frame._partitions]
-                images, image = gk.key_image(keys)
-                if image is not None:
-                    pc = by_frame._partition_mgr_cls._partition_class
-                    by_frame = type(by_frame)(np.array([[pc(b)] for b in images], dtype=object), by_frame.copy_index_cache(),
-                                              images[0].columns, by_frame.row_lengths, [1])  # fmt: skip
-                if drop and len(by.columns) > 1:  # the packed key has a label of its own: the key columns leave here
-                    keep = [c for c in query_compiler.columns if c not in set(by.columns)]
-                    frame = query_compiler.getitem_column_array(keep)._modin_frame
-                # the functors themselves, not lambdas around them: the partition manager recognises them and fuses
-                # map + reduce into one direct-addressed table per GPU when the key range allows (pm.groupby_reduce)
-                new_frame = frame.groupby_reduce(axis, by_frame, map_f, red_f)
-                if image is not None or level is not None:
-                    # the private key label of groupby(level=) gives way to the index level's own name
-                    blocks = gk.restore_keys([row[0].get() for row in new_frame._partitions], image,
-                                             groupby_kwargs.get("dropna", True), [level_name] if level is not None else None)
-                    pc = new_frame._partition_mgr_cls._partition_class
-                    new_frame = type(new_frame)(np.array([[pc(b)] for b in blocks], dtype=object), None, None, None, None)
-                if not groupby_kwargs.get("as_index", True):
-                    from .query_compiler import group_keys_to_columns
+                by, name = _labels_as_by(query_compiler, level)
+                key_names = [name]
+            return groupby_agg(query_compiler, by, axis, groupby_kwargs, agg_args, agg_kwargs, drop=drop,
+                               key_names=key_names, **kwargs)  # fmt: skip
 
-                    new_frame = group_keys_to_columns(new_frame)  # alg/groupby.py:278-294
-                return query_compiler.__constructor__(new_frame)
-
-            return caller
+        return caller
 
     # ---------------------------------------------------------------- query compiler
-    _f64 = lambda *a, **k: np.dtype("float64")  # noqa: E731
-
-    def _arith(op):
-        """``Binary.register(DevBinary(op), infer_dtypes="common_cast")`` (qc.py:535-566) with one shortcut in front:
+    def _arith(op, generic):
+        """The ``generic`` Binary registration of ``op`` (qc.py:535-566) with one shortcut in front:
         a float64 frame against a real SCALAR keeps its dtypes, so the template's dtype inference (a pandas concat of
         two dtype Series per operator, ~0.5 ms of host time: as much as the kernel needs for 2e7 rows) is skipped and
         the scalar branch of the template (alg/binary.py:444-455: a lazy ``frame.map``) is taken directly."""
-        generic = Binary.register(fx.DevBinary(op), infer_dtypes="common_cast")
         functor = fx.DevBinary(op)
 
         def caller(query_compiler, other, broadcast=False, *args, dtypes=None, **kwargs):
@@ -425,7 +390,9 @@ def register(shims: bool | None = None):
 
         return caller
 
-    class B200OnModinQueryCompiler(PandasQueryCompiler):
+    Ops = device_operations(malg)
+
+    class B200OnModinQueryCompiler(Ops, PandasQueryCompiler):
         def get_axis_len(self, axis):
             """qc.py:411-427.  Under torch.distributed ``len(df)`` is the JOB-wide row count, not this rank's shard:
             Modin's API layer decides from it whether a frame is ``empty`` -- and defaults every method call on an
@@ -447,130 +414,30 @@ def register(shims: bool | None = None):
                 return n
             return super().get_axis_len(axis)
 
-        # Map (qc.py:2036-2106)
-        abs = Map.register(fx.DevMap("abs"), dtypes="copy")
-        negative = Map.register(fx.DevMap("neg"), dtypes="copy")
-        isna = Map.register(fx.DevMap("isna"), dtypes=np.bool_)
-        notna = Map.register(fx.DevMap("notna"), dtypes=np.bool_)
-        round = Map.register(fx.DevRound(), dtypes="copy")  # qc.py:2438
-        clip = Map.register(fx.DevClip(), dtypes="copy")
         # Binary (qc.py:535-624)
-        add = _arith("add")
-        radd = _arith("radd")
-        sub = _arith("sub")
-        rsub = _arith("rsub")
-        mul = _arith("mul")
-        rmul = _arith("rmul")
-        truediv = _arith("truediv")
-        rtruediv = _arith("rtruediv")
-        eq = Binary.register(fx.DevBinary("eq"), infer_dtypes="bool")
-        ne = Binary.register(fx.DevBinary("ne"), infer_dtypes="bool")
-        lt = Binary.register(fx.DevBinary("lt"), infer_dtypes="bool")
-        le = Binary.register(fx.DevBinary("le"), infer_dtypes="bool")
-        gt = Binary.register(fx.DevBinary("gt"), infer_dtypes="bool")
-        ge = Binary.register(fx.DevBinary("ge"), infer_dtypes="bool")
+        add = _arith("add", Ops.add)
+        radd = _arith("radd", Ops.radd)
+        sub = _arith("sub", Ops.sub)
+        rsub = _arith("rsub", Ops.rsub)
+        mul = _arith("mul", Ops.mul)
+        rmul = _arith("rmul", Ops.rmul)
+        truediv = _arith("truediv", Ops.truediv)
+        rtruediv = _arith("rtruediv", Ops.rtruediv)
         # Series comparisons are separate registrations in the reference (qc.py:586-604, they take fill_value);
         # on the device a Series is a one-column frame, so the same functors serve
-        series_eq = Binary.register(fx.DevBinary("eq"), infer_dtypes="bool")
-        series_ne = Binary.register(fx.DevBinary("ne"), infer_dtypes="bool")
-        series_lt = Binary.register(fx.DevBinary("lt"), infer_dtypes="bool")
-        series_le = Binary.register(fx.DevBinary("le"), infer_dtypes="bool")
-        series_gt = Binary.register(fx.DevBinary("gt"), infer_dtypes="bool")
-        series_ge = Binary.register(fx.DevBinary("ge"), infer_dtypes="bool")
-        __and__ = Binary.register(fx.DevLogical("and"), infer_dtypes="bool")  # qc.py:541-571
-        __or__ = Binary.register(fx.DevLogical("or"), infer_dtypes="bool")
-        __xor__ = Binary.register(fx.DevLogical("xor"), infer_dtypes="bool")
-        invert = Map.register(fx.DevMap("not"), dtypes=np.bool_)
-        # TreeReduce (qc.py:976-1096)
-        count = TreeReduce.register(fx.DevReduce("count"), fx.DevReduce("count", phase="reduce"),
-                                    compute_dtypes=lambda *a, **k: np.dtype("int64"))  # fmt: skip
-        sum = TreeReduce.register(fx.DevReduce("sum"), fx.DevReduce("sum", phase="reduce"), compute_dtypes=_dtypes_sum)
-        max = TreeReduce.register(fx.DevReduce("max"), fx.DevReduce("max", phase="reduce"))
-        min = TreeReduce.register(fx.DevReduce("min"), fx.DevReduce("min", phase="reduce"))
-        mean = TreeReduce.register(fx.DevMeanMap(), fx.DevMeanReduce(), compute_dtypes=_f64)
-        prod = TreeReduce.register(fx.DevReduce("prod"), fx.DevReduce("prod", phase="reduce"), compute_dtypes=_dtypes_sum)
-        any = TreeReduce.register(fx.DevBoolReduce("any"), fx.DevBoolReduce("any", phase="reduce"),
-                                  compute_dtypes=lambda *a, **k: np.dtype("bool"))  # qc.py:986
-        all = TreeReduce.register(fx.DevBoolReduce("all"), fx.DevBoolReduce("all", phase="reduce"),
-                                  compute_dtypes=lambda *a, **k: np.dtype("bool"))  # qc.py:987
-        # GroupByReduce (qc.py:3741-3748)
-        groupby_sum = B200GroupByReduce.register_agg("sum")
-        groupby_count = B200GroupByReduce.register_agg("count")
-        groupby_size = B200GroupByReduce.register_agg("size")
-        groupby_mean = B200GroupByReduce.register_agg("mean")
-        groupby_min = B200GroupByReduce.register_agg("min")
-        groupby_max = B200GroupByReduce.register_agg("max")
-
-        _DEVICE_AGGS = ("sum", "count", "size", "mean", "min", "max")
-
-        def groupby_agg(self, by, agg_func, axis, groupby_kwargs, agg_args, agg_kwargs, how="axis_wise", drop=False,
-                        series_groupby=False):  # fmt: skip
-            """qc.py:4236-4527.  The reference sends ``{column: function}`` dictionaries whose functions all have a
-            map / reduce form through ``_groupby_dict_reduce`` (qc.py:3876-3970: one map table and one reduce table
-            per function) and everything else through a full-axis ``groupby.agg`` on pandas blocks.  Here a dictionary
-            over the device aggregations becomes one device aggregation per DISTINCT function over the columns that
-            ask for it; every result carries the same ascending group keys, so the result blocks are zipped
-            column-wise (buffers shared) in the dictionary's order.  A function name alone goes to its registered
-            template.  Anything else has no device form and is refused -- there is no pandas block to fall back to."""
-            if how != "axis_wise" or agg_args or agg_kwargs:
-                raise NotImplementedError(f"groupby ({how}) with extra arguments is not on the B200 path")
-            if isinstance(agg_func, str) and agg_func in self._DEVICE_AGGS:
-                return getattr(self, f"groupby_{agg_func}")(
-                    by=by, axis=axis, groupby_kwargs=groupby_kwargs, agg_args=agg_args, agg_kwargs=agg_kwargs, drop=drop
-                )
-            if not isinstance(agg_func, dict) or not agg_func:
-                raise NotImplementedError(f"groupby.agg({agg_func!r}) is not on the B200 path")
-            if not isinstance(by, type(self)):
-                raise NotImplementedError("device groupby: key columns of the same frame, axis=0")
-            spec = {col: fn[0] if isinstance(fn, (list, tuple)) and len(fn) == 1 else fn for col, fn in agg_func.items()}
-            by_func = gk.split_aggregations(spec, self.columns, set(by.columns) if drop else ())
-            if any(isinstance(fn, (list, tuple)) for fn in agg_func.values()):
-                raise NotImplementedError("groupby.agg with lists of functions (two-level result columns)")
-            kw = dict(groupby_kwargs, as_index=True)
-            results = []
-            for fn, cols in by_func.items():
-                res = getattr(self.getitem_column_array(cols), f"groupby_{fn}")(
-                    by=by, axis=axis, groupby_kwargs=kw, agg_args=(), agg_kwargs={}, drop=False
-                )
-                results.append([[p.get() for p in row] for row in res._modin_frame._partitions])
-            pc = self._modin_frame._partition_mgr_cls._partition_class
-            rows = [[pc(b)] for b in gk.zip_aggregations(spec, by_func, results)]
-            new_frame = type(self._modin_frame)(np.array(rows, dtype=object), None, None, None, None)
-            if not groupby_kwargs.get("as_index", True):
-                from .query_compiler import group_keys_to_columns
-
-                new_frame = group_keys_to_columns(new_frame)  # alg/groupby.py:278-294
-            return self.__constructor__(new_frame)
-
-        def fillna(self, **kwargs):
-            """qc.py:2710-2813."""
-            value = kwargs.get("value")
-            if kwargs.get("method") is not None:  # qc.py:2809-2810: a Fold
-                if kwargs["method"] not in ("ffill", "pad") or value is not None or kwargs.get("limit") is not None \
-                        or kwargs.get("axis") not in (0, "index", None):  # fmt: skip
-                    raise NotImplementedError("fillna(method=) on the B200 path: forward fill down the rows, no limit=")
-                return self._ffill(0)
-            if kwargs.get("limit") is not None:
-                raise NotImplementedError("fillna(limit=) is not on the B200 path")
-            if isinstance(value, type(self)):
-                return self.__constructor__(
-                    # PandasDataframe.n_ary_op takes the dtypes themselves: the "copy" shorthand is only understood by
-                    # the Binary template and broadcast_apply (it used to reach ModinDtypes as a string and fail)
-                    self._modin_frame.n_ary_op(lambda x, y: fx.DevBinary("fillna")(x, y), [value._modin_frame],
-                                               join_type="left", dtypes=self._modin_frame.copy_dtypes_cache())
-                )  # fmt: skip
-            kw = {k: v for k, v in kwargs.items() if k in ("value",)}
-            return self.__constructor__(self._modin_frame.map(lambda x: fx.DevFillna()(x, **kw), dtypes="copy"))
-
-        def astype(self, col_dtypes, errors: str = "raise"):
-            """qc.py:2335-2343 -> PandasDataframe.astype (df.py:1707-1810) maps ``df.astype`` over the blocks; here the
-            block function is the device cast (widening casts only, checked before anything is launched)."""
-            if errors != "raise":
-                raise NotImplementedError("astype(errors='ignore') is not on the B200 path")
-            mapping = fx.DevAstype.validate(self.dtypes, col_dtypes)
-            fn = fx.DevAstype()
-            return self.__constructor__(self._modin_frame.map(lambda blk: fn(blk, col_dtypes=mapping)),
-                                        shape_hint=self._shape_hint)  # fmt: skip
+        series_eq = malg.Binary.register(fx.DevBinary("eq"), infer_dtypes="bool")
+        series_ne = malg.Binary.register(fx.DevBinary("ne"), infer_dtypes="bool")
+        series_lt = malg.Binary.register(fx.DevBinary("lt"), infer_dtypes="bool")
+        series_le = malg.Binary.register(fx.DevBinary("le"), infer_dtypes="bool")
+        series_gt = malg.Binary.register(fx.DevBinary("gt"), infer_dtypes="bool")
+        series_ge = malg.Binary.register(fx.DevBinary("ge"), infer_dtypes="bool")
+        # GroupByReduce (qc.py:3741-3748), with groupby(level=)
+        groupby_sum = _by_level(Ops.groupby_sum)
+        groupby_count = _by_level(Ops.groupby_count)
+        groupby_size = _by_level(Ops.groupby_size)
+        groupby_mean = _by_level(Ops.groupby_mean)
+        groupby_min = _by_level(Ops.groupby_min)
+        groupby_max = _by_level(Ops.groupby_max)
 
         def unique(self, keep="first", ignore_index=True, subset=None):
             """qc.py:2231-2270 -- what ``drop_duplicates`` (modin/pandas/base.py:1600-1623) and ``Series.unique``
@@ -673,21 +540,6 @@ def register(shims: bool | None = None):
             )  # fmt: skip
             return self.getitem_array(self.__constructor__(mask, shape_hint="column"))
 
-        # qc.py:1155-1156: std / var = Reduce.register(pandas.DataFrame.std / var) -- same template, device functor
-        # (two sweeps over each full column partition, two packed all-reduces when the rows span ranks)
-        # qc.py:1101-1102: idxmax / idxmin = Reduce.register(pandas.DataFrame.idxmax / idxmin) -- one arg-reduction
-        # pass per column partition, one W-vector all-gather when the rows span ranks
-        idxmax = Reduce.register(fx.DevArgReduce("max"))
-        idxmin = Reduce.register(fx.DevArgReduce("min"))
-        var = Reduce.register(fx.DevVar(sqrt=False))
-        std = Reduce.register(fx.DevVar(sqrt=True))
-        # qc.py:2429-2431: cumulative functions through the Fold template (csrc/cum.cu); forward fill rides the same
-        # scan (fillna(method="ffill"), qc.py:2809-2810)
-        cumsum = Fold.register(fx.DevCumulative("sum"), shape_preserved=True)
-        cummax = Fold.register(fx.DevCumulative("max"), shape_preserved=True)
-        cummin = Fold.register(fx.DevCumulative("min"), shape_preserved=True)
-        _ffill = Fold.register(fx.DevCumulative("ffill"), shape_preserved=True)
-
         def cumprod(self, *args, **kwargs):
             raise NotImplementedError("cumprod is not on the B200 path")
 
@@ -696,18 +548,7 @@ def register(shims: bool | None = None):
             (metadata).  Turning row labels into columns would need the labels on the device first."""
             if not kwargs.get("drop", False) or kwargs.get("level") is not None:
                 raise NotImplementedError("reset_index on the B200 path: drop=True, no level=")
-            from .query_compiler import _reset_row_index
-
             return self.__constructor__(_reset_row_index(self._modin_frame))
-
-        def merge(self, right, **kwargs):
-            """qc.py:657-667 -> MergeImpl.row_axis_merge (merge.py:104-252) with the per-block ``pandas.merge``
-            replaced by the device join functor (``modin_b200.merge``): many-to-one and many-to-many keys,
-            ``on`` or ``left_on`` / ``right_on``, how in {left, inner}."""
-            from .merge import row_axis_merge
-            from .query_compiler import _reset_row_index
-
-            return self.__constructor__(row_axis_merge(self, right, _reset_row_index, **kwargs))
 
     # ---------------------------------------------------------------- IO + factory
     class B200IO(BaseIO):

@@ -18,10 +18,9 @@ from typing import Optional
 import numpy as np
 import pandas
 
-from .. import groupkeys as gk
 from ..functors import MODIN_UNNAMED_SERIES_LABEL
 from ..dataframe import B200Dataframe
-from ..query_compiler import B200QueryCompiler, group_keys_to_columns
+from ..query_compiler import B200QueryCompiler
 
 
 def _is_scalar(x):
@@ -399,29 +398,21 @@ class DataFrame(BasePandasDataset):
             raise NotImplementedError("groupby(axis=1) is not on the B200 path")
         if level is not None:
             raise NotImplementedError("groupby(level=) is not on the B200 path")
-        if as_index not in (True, False):  # the aggregations ask the template for as_index=True and apply it themselves
-            raise NotImplementedError(f"groupby(as_index={as_index!r}) is not on the B200 path")
+        for key, value, allowed in (("as_index", as_index, (True, False)), ("observed", observed, (True, False, None))):
+            if value not in allowed:
+                raise NotImplementedError(f"groupby({key}={value!r}) is not on the B200 path")
         kwargs = dict(as_index=as_index, sort=sort, group_keys=group_keys, observed=observed, dropna=dropna, level=level)
         if isinstance(by, (list, tuple)) and len(by) != 1:
-            # several int64 keys: the groupby runs on their packed image, which takes the key columns' place
-            from ..block import DeviceBlock, concat_cols
-
+            # several int64 keys: the query compiler groups by their packed image, and drops the key columns
             for k in by:
                 if k not in self.columns:
                     raise KeyError(k)
             if len(set(by)) != len(by):
                 raise ValueError("duplicate key columns")
-            frame = self._query_compiler._modin_frame
-            rows = [concat_cols([p.get() for p in row]) if len(row) > 1 else row[0].get() for row in frame._partitions]
-            pos = [int(self.columns.get_loc(k)) for k in by]
-            images, image = gk.key_image([b.select_columns(pos) for b in rows])
-            keep = [j for j in range(len(self.columns)) if j not in pos]
-            labels = pandas.Index([self.columns[j] for j in keep] + [gk.PACKED_KEY])
-            blocks = [DeviceBlock([b.cols[j] for j in keep] + img.cols, labels, nrows=b.nrows, range_start=b.range_start)
-                      for b, img in zip(rows, images)]  # fmt: skip
-            packed = DataFrame(query_compiler=type(self._query_compiler)(B200Dataframe.from_blocks(blocks)))
-            return DataFrameGroupBy(packed, packed[gk.PACKED_KEY]._query_compiler, drop=True, groupby_kwargs=kwargs,
-                                    image=image)  # fmt: skip
+            if any(np.dtype(self.dtypes[k]) != np.int64 for k in by):
+                raise NotImplementedError("multi-column groupby on the B200 path needs int64 key columns")
+            return DataFrameGroupBy(self, self._query_compiler.getitem_column_array(list(by)), drop=True,
+                                    groupby_kwargs=kwargs)  # fmt: skip
         if isinstance(by, (list, tuple)):
             by = by[0]
         drop = False
@@ -590,26 +581,22 @@ class Series(BasePandasDataset):
 class DataFrameGroupBy:
     """modin/pandas/groupby.py (``_wrap_aggregation`` :1829-1886)."""
 
-    def __init__(self, df: DataFrame, by_qc, drop, groupby_kwargs, image=None):
+    def __init__(self, df: DataFrame, by_qc, drop, groupby_kwargs):
         self._df = df
         self._query_compiler = df._query_compiler
         self._by = by_qc
         self._drop = drop
         self._kwargs = groupby_kwargs
-        self._image = image  # how the keys behind ``by_qc`` are restored (``groupkeys.key_image``)
+
+    def _check_keys(self):
+        if len(self._by.columns) == 1 and self._by.dtypes.iloc[0] == np.float64:  # float keys are not on this front door
+            raise NotImplementedError("device groupby needs an int64 key column")
 
     def _wrap_aggregation(self, qc_method, numeric_only=False, agg_args=None, agg_kwargs=None):
-        result_qc = qc_method(self._query_compiler, by=self._by, axis=0, groupby_kwargs=dict(self._kwargs, as_index=True),
+        self._check_keys()
+        result_qc = qc_method(self._query_compiler, by=self._by, axis=0, groupby_kwargs=self._kwargs,
                               agg_args=agg_args or [], agg_kwargs=agg_kwargs or {}, drop=self._drop)  # fmt: skip
-        return self._finish(result_qc._modin_frame)
-
-    def _finish(self, frame):
-        """The result with the original keys restored, then -- ``as_index=False`` -- turned into leading columns."""
-        if self._image is not None:
-            frame = B200Dataframe.from_blocks(gk.restore_keys([row[0].get() for row in frame._partitions], self._image))
-        if not self._kwargs.get("as_index", True):
-            frame = group_keys_to_columns(frame)  # alg/groupby.py:278-294
-        return DataFrame(query_compiler=type(self._query_compiler)(frame))
+        return DataFrame(query_compiler=result_qc)
 
     def sum(self, numeric_only=False, min_count=0):
         if min_count:
@@ -642,17 +629,12 @@ class DataFrameGroupBy:
     def _dict_agg(self, spec):
         """``groupby(key).agg({column: function})`` -- qc._groupby_dict_reduce (qc.py:3876-3970) splits a dictionary
         aggregation into per-function map / reduce tables.  Here: one device aggregation per distinct function over
-        the columns that ask for it, zipped column-wise in the dictionary's order (``groupkeys.zip_aggregations``)."""
+        the columns that ask for it, zipped column-wise in the dictionary's order (``qc.groupby_agg``)."""
         if not self._drop:
             raise NotImplementedError("dictionary aggregation needs the key column inside the frame")
-        key = self._by.columns[0]
-        by_func = gk.split_aggregations(spec, self._df.columns, (key,))
-        kw = dict(self._kwargs, as_index=True)
-        results = []
-        for fn, cols in by_func.items():
-            res = getattr(self._df[[key] + cols].groupby(key, **kw), fn)()
-            results.append([[p.get() for p in row] for row in res._query_compiler._modin_frame._partitions])
-        return self._finish(B200Dataframe.from_blocks(gk.zip_aggregations(spec, by_func, results)))
+        self._check_keys()
+        return DataFrame(query_compiler=self._query_compiler.groupby_agg(self._by, spec, 0, self._kwargs, (), {},
+                                                                         drop=self._drop))  # fmt: skip
 
     aggregate = agg
 

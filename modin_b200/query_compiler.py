@@ -1,5 +1,11 @@
-"""B200QueryCompiler: the hot-path subset of PandasQueryCompiler with device functors registered
-through the operator templates.
+"""The device surface both query compilers share, and ``B200QueryCompiler``, the Modin-free one that holds a
+``B200Dataframe``.
+
+``device_operations(alg)`` returns the one definition of every device operation: the Map / Binary / TreeReduce /
+Reduce / Fold registrations with their device functors, ``fillna`` / ``astype`` / ``merge``, and the groupby
+aggregations.  ``alg`` is the module of operator templates the registrations go through: ``modin_b200.algebra`` for
+the mirror below, ``modin.core.dataframe.algebra`` for the Modin plug-in (``modin_plugin.py``), whose query compiler
+puts the class in front of ``PandasQueryCompiler`` so that these entries replace Modin's.
 
 Reference registrations being mirrored (modin/core/storage_formats/pandas/query_compiler.py):
 Binary ops ``:535-624``; ``count/sum/max/min/mean`` TreeReduce ``:976-1096``; ``abs`` ``:2036``;
@@ -17,7 +23,9 @@ from __future__ import annotations
 import numpy as np
 import pandas
 
-from .algebra import Binary, Fold, GroupByReduce, Map, Reduce, TreeReduce
+from . import algebra
+from . import groupkeys as gk
+from .block import concat_cols
 from .dataframe import B200Dataframe
 from .functors import (
     DevArgReduce,
@@ -37,7 +45,6 @@ from .functors import (
     DevRound,
     DevVar,
 )
-from .partitioning import Bound
 
 
 def _dtypes_sum(dtypes: pandas.Series, *func_args, **func_kwargs):
@@ -45,7 +52,190 @@ def _dtypes_sum(dtypes: pandas.Series, *func_args, **func_kwargs):
     return np.result_type(*dtypes.values) if len(dtypes) else np.dtype("float64")
 
 
-class B200QueryCompiler:
+def _groupby_reduce(agg: str):
+    """``qc.groupby_<agg>`` (qc.py:3741-3748, alg/groupby.py) over device blocks.  ``by`` is a query compiler of key
+    columns with the frame's rows; ``key_names`` replaces the names of the result's keys (``groupby(level=)``)."""
+    map_f, red_f = DevGroupbyMap(agg), DevGroupbyReduce(agg)
+
+    def caller(query_compiler, by, axis, groupby_kwargs, agg_args, agg_kwargs, drop=False, key_names=None, **kwargs):
+        if axis != 0 or not isinstance(by, type(query_compiler)) or len(by.columns) < 1:
+            raise NotImplementedError("device groupby: key columns of the same frame, axis=0")
+        frame, by_frame = query_compiler._modin_frame, by._modin_frame
+        # a float64 key or several int64 keys: the single-key groupby runs on their int64 image and the G result keys
+        # are restored afterwards (groupkeys.py); one int64 key is its own image
+        keys = [concat_cols([p.get() for p in row]) if len(row) > 1 else row[0].get() for row in by_frame._partitions]
+        images, image = gk.key_image(keys)
+        if image is not None:
+            pc = by_frame._partition_mgr_cls._partition_class
+            by_frame = type(by_frame)(np.array([[pc(b)] for b in images], dtype=object), by_frame.copy_index_cache(),
+                                      images[0].columns, by_frame.row_lengths, [1])  # fmt: skip
+        if drop and len(by.columns) > 1:  # the packed key has a label of its own: the key columns leave here
+            keep = [c for c in query_compiler.columns if c not in set(by.columns)]
+            frame = query_compiler.getitem_column_array(keep)._modin_frame
+        # the functors themselves, not lambdas around them: the partition manager recognises them and fuses map +
+        # reduce into one direct-addressed table per GPU when the key range allows (pm.groupby_reduce)
+        new_frame = frame.groupby_reduce(axis, by_frame, map_f, red_f)
+        if image is not None or key_names is not None:
+            blocks = gk.restore_keys([row[0].get() for row in new_frame._partitions], image,
+                                     groupby_kwargs.get("dropna", True), key_names)  # fmt: skip
+            pc = new_frame._partition_mgr_cls._partition_class
+            new_frame = type(new_frame)(np.array([[pc(b)] for b in blocks], dtype=object), None, None, None, None)
+        if not groupby_kwargs.get("as_index", True):
+            new_frame = group_keys_to_columns(new_frame)  # alg/groupby.py:278-294
+        return query_compiler.__constructor__(new_frame)
+
+    return caller
+
+
+def device_operations(alg):
+    """The device operations of a query compiler, registered through the operator templates of ``alg``."""
+
+    class DeviceOperations:
+        # ---- Map (qc.py:2036-2106) ----------------------------------------------------------------------
+        abs = alg.Map.register(DevMap("abs"), dtypes="copy")
+        negative = alg.Map.register(DevMap("neg"), dtypes="copy")
+        isna = alg.Map.register(DevMap("isna"), dtypes=np.bool_)
+        notna = alg.Map.register(DevMap("notna"), dtypes=np.bool_)
+        round = alg.Map.register(DevRound(), dtypes="copy")  # qc.py:2438
+        clip = alg.Map.register(DevClip(), dtypes="copy")  # qc.py `clip = Map.register(pandas.DataFrame.clip)`
+        invert = alg.Map.register(DevMap("not"), dtypes=np.bool_)
+        _astype_map = alg.Map.register(DevAstype())  # result dtypes are read back from the blocks
+
+        def astype(self, col_dtypes, errors: str = "raise"):
+            """qc.py ``astype(col_dtypes, errors)``: ``col_dtypes`` is one dtype for every column or a
+            {column label: dtype} mapping.  Only the widening casts of ``DevAstype``; checked here, before any launch,
+            so that a refused cast leaves no half-converted frame."""
+            if errors != "raise":
+                raise NotImplementedError("astype(errors='ignore') is not on the B200 path")
+            return self._astype_map(col_dtypes=DevAstype.validate(self.dtypes, col_dtypes))
+
+        def fillna(self, **kwargs):
+            """qc.py:2710-2813: scalar / dict values are a Map, a frame value is an n-ary op; forward fill is a Fold."""
+            value = kwargs.get("value")
+            if kwargs.get("method") is not None:  # qc.py:2809-2810
+                if kwargs["method"] not in ("ffill", "pad") or value is not None or kwargs.get("limit") is not None \
+                        or kwargs.get("axis") not in (0, "index", None):  # fmt: skip
+                    raise NotImplementedError("fillna(method=) on the B200 path: forward fill down the rows, no limit=")
+                return self._ffill(0)
+            if kwargs.get("limit") is not None:
+                raise NotImplementedError("fillna(limit=) is not on the B200 path")
+            if isinstance(value, type(self)):
+                return self.__constructor__(
+                    # PandasDataframe.n_ary_op takes the dtypes themselves: the "copy" shorthand is only understood by
+                    # the Binary template and broadcast_apply
+                    self._modin_frame.n_ary_op(lambda x, y: DevBinary("fillna")(x, y), [value._modin_frame],
+                                               join_type="left", dtypes=self._modin_frame.copy_dtypes_cache())
+                )  # fmt: skip
+            return self.__constructor__(self._modin_frame.map(lambda x: DevFillna()(x, value=value), dtypes="copy"))
+
+        # ---- Binary (qc.py:535-624) ---------------------------------------------------------------------
+        add = alg.Binary.register(DevBinary("add"), infer_dtypes="common_cast")
+        radd = alg.Binary.register(DevBinary("radd"), infer_dtypes="common_cast")
+        sub = alg.Binary.register(DevBinary("sub"), infer_dtypes="common_cast")
+        rsub = alg.Binary.register(DevBinary("rsub"), infer_dtypes="common_cast")
+        mul = alg.Binary.register(DevBinary("mul"), infer_dtypes="common_cast")
+        rmul = alg.Binary.register(DevBinary("rmul"), infer_dtypes="common_cast")
+        truediv = alg.Binary.register(DevBinary("truediv"), infer_dtypes="common_cast")
+        rtruediv = alg.Binary.register(DevBinary("rtruediv"), infer_dtypes="common_cast")
+        eq = alg.Binary.register(DevBinary("eq"), infer_dtypes="bool")
+        ne = alg.Binary.register(DevBinary("ne"), infer_dtypes="bool")
+        lt = alg.Binary.register(DevBinary("lt"), infer_dtypes="bool")
+        le = alg.Binary.register(DevBinary("le"), infer_dtypes="bool")
+        gt = alg.Binary.register(DevBinary("gt"), infer_dtypes="bool")
+        ge = alg.Binary.register(DevBinary("ge"), infer_dtypes="bool")
+        # logical ops between bool frames (qc.py:541-571)
+        __and__ = alg.Binary.register(DevLogical("and"), infer_dtypes="bool")
+        __or__ = alg.Binary.register(DevLogical("or"), infer_dtypes="bool")
+        __xor__ = alg.Binary.register(DevLogical("xor"), infer_dtypes="bool")
+
+        # ---- TreeReduce (qc.py:976-1096) ----------------------------------------------------------------
+        count = alg.TreeReduce.register(DevReduce("count"), DevReduce("count", phase="reduce"),
+                                        compute_dtypes=lambda *a, **k: np.dtype("int64"))  # fmt: skip
+        sum = alg.TreeReduce.register(DevReduce("sum"), DevReduce("sum", phase="reduce"), compute_dtypes=_dtypes_sum)
+        prod = alg.TreeReduce.register(DevReduce("prod"), DevReduce("prod", phase="reduce"), compute_dtypes=_dtypes_sum)
+        max = alg.TreeReduce.register(DevReduce("max"), DevReduce("max", phase="reduce"))
+        min = alg.TreeReduce.register(DevReduce("min"), DevReduce("min", phase="reduce"))
+        mean = alg.TreeReduce.register(DevMeanMap(), DevMeanReduce(), compute_dtypes=lambda *a, **k: np.dtype("float64"))
+        any = alg.TreeReduce.register(DevBoolReduce("any"), DevBoolReduce("any", phase="reduce"),
+                                      compute_dtypes=lambda *a, **k: np.dtype("bool"))  # qc.py:986
+        all = alg.TreeReduce.register(DevBoolReduce("all"), DevBoolReduce("all", phase="reduce"),
+                                      compute_dtypes=lambda *a, **k: np.dtype("bool"))  # qc.py:987
+
+        # ---- Reduce: one function over FULL column partitions ---------------------------------------------
+        # qc.py:1155-1156: std / var = Reduce.register(pandas.DataFrame.std / var) -- two sweeps over each full column
+        # partition, two packed all-reduces when the rows span ranks
+        # qc.py:1101-1102: idxmax / idxmin = Reduce.register(pandas.DataFrame.idxmax / idxmin) -- one arg-reduction
+        # pass per column partition, one W-vector all-gather when the rows span ranks
+        idxmax = alg.Reduce.register(DevArgReduce("max"))
+        idxmin = alg.Reduce.register(DevArgReduce("min"))
+        var = alg.Reduce.register(DevVar(sqrt=False))
+        std = alg.Reduce.register(DevVar(sqrt=True))
+
+        # ---- Fold (qc.py:2429-2431; forward fill is fillna(method="ffill"), qc.py:2809-2810) ----------------------
+        cumsum = alg.Fold.register(DevCumulative("sum"), shape_preserved=True)
+        cummax = alg.Fold.register(DevCumulative("max"), shape_preserved=True)
+        cummin = alg.Fold.register(DevCumulative("min"), shape_preserved=True)
+        _ffill = alg.Fold.register(DevCumulative("ffill"), shape_preserved=True)
+
+        # ---- GroupByReduce (qc.py:3741-3748; impl table storage_formats/pandas/groupby.py:237-248) ------
+        groupby_sum = _groupby_reduce("sum")
+        groupby_count = _groupby_reduce("count")
+        groupby_size = _groupby_reduce("size")
+        groupby_mean = _groupby_reduce("mean")
+        groupby_min = _groupby_reduce("min")
+        groupby_max = _groupby_reduce("max")
+
+        _DEVICE_AGGS = ("sum", "count", "size", "mean", "min", "max")
+
+        def groupby_agg(self, by, agg_func, axis, groupby_kwargs, agg_args, agg_kwargs, how="axis_wise", drop=False,
+                        series_groupby=False):  # fmt: skip
+            """qc.py:4236-4527.  The reference sends ``{column: function}`` dictionaries whose functions all have a
+            map / reduce form through ``_groupby_dict_reduce`` (qc.py:3876-3970: one map table and one reduce table
+            per function) and everything else through a full-axis ``groupby.agg`` on pandas blocks.  Here a dictionary
+            over the device aggregations becomes one device aggregation per DISTINCT function over the columns that
+            ask for it; every result carries the same ascending group keys, so the result blocks are zipped
+            column-wise (buffers shared) in the dictionary's order.  A function name alone goes to its registered
+            template.  Anything else has no device form and is refused -- there is no pandas block to fall back to."""
+            if how != "axis_wise" or agg_args or agg_kwargs:
+                raise NotImplementedError(f"groupby ({how}) with extra arguments is not on the B200 path")
+            if isinstance(agg_func, str) and agg_func in self._DEVICE_AGGS:
+                return getattr(self, f"groupby_{agg_func}")(
+                    by=by, axis=axis, groupby_kwargs=groupby_kwargs, agg_args=agg_args, agg_kwargs=agg_kwargs, drop=drop
+                )
+            if not isinstance(agg_func, dict) or not agg_func:
+                raise NotImplementedError(f"groupby.agg({agg_func!r}) is not on the B200 path")
+            if not isinstance(by, type(self)):
+                raise NotImplementedError("device groupby: key columns of the same frame, axis=0")
+            spec = {col: fn[0] if isinstance(fn, (list, tuple)) and len(fn) == 1 else fn for col, fn in agg_func.items()}
+            by_func = gk.split_aggregations(spec, self.columns, set(by.columns) if drop else ())
+            if any(isinstance(fn, (list, tuple)) for fn in agg_func.values()):
+                raise NotImplementedError("groupby.agg with lists of functions (two-level result columns)")
+            kw = dict(groupby_kwargs, as_index=True)
+            results = []
+            for fn, cols in by_func.items():
+                res = getattr(self.getitem_column_array(cols), f"groupby_{fn}")(
+                    by=by, axis=axis, groupby_kwargs=kw, agg_args=(), agg_kwargs={}, drop=False
+                )
+                results.append([[p.get() for p in row] for row in res._modin_frame._partitions])
+            pc = self._modin_frame._partition_mgr_cls._partition_class
+            rows = [[pc(b)] for b in gk.zip_aggregations(spec, by_func, results)]
+            new_frame = type(self._modin_frame)(np.array(rows, dtype=object), None, None, None, None)
+            if not groupby_kwargs.get("as_index", True):
+                new_frame = group_keys_to_columns(new_frame)  # alg/groupby.py:278-294
+            return self.__constructor__(new_frame)
+
+        # ---- merge (qc.py:657-667 -> MergeImpl.row_axis_merge merge.py:104-252) --------------------------
+        def merge(self, right, **kwargs):
+            """The per-block ``pandas.merge`` replaced by the device join functor (``modin_b200.merge``): many-to-one
+            and many-to-many keys, ``on`` or ``left_on`` / ``right_on``, how in {left, inner}."""
+            from .merge import row_axis_merge
+
+            return self.__constructor__(row_axis_merge(self, right, _reset_row_index, **kwargs))
+
+    return DeviceOperations
+
+
+class B200QueryCompiler(device_operations(algebra)):
     """Query compiler holding a ``B200Dataframe`` (qc.py:279-302)."""
 
     _modin_frame: B200Dataframe
@@ -181,111 +371,18 @@ class B200QueryCompiler:
                 raise KeyError(f"{missing} not in index")
         return self.__constructor__(self._modin_frame.take_2d_labels_or_positional(col_positions=positions))
 
-    # ---- Map (qc.py:2036-2106) ----------------------------------------------------------------------
-    abs = Map.register(DevMap("abs"), dtypes="copy")
-    negative = Map.register(DevMap("neg"), dtypes="copy")
-    isna = Map.register(DevMap("isna"), dtypes=np.bool_)
-    notna = Map.register(DevMap("notna"), dtypes=np.bool_)
-    round = Map.register(DevRound(), dtypes="copy")  # qc.py:2438
-    clip = Map.register(DevClip(), dtypes="copy")  # qc.py `clip = Map.register(pandas.DataFrame.clip)`
-    copy_data = Map.register(DevMap("copy"), dtypes="copy")
-    _astype_map = Map.register(DevAstype())  # result dtypes are read back from the blocks
-
-    def astype(self, col_dtypes, errors: str = "raise"):
-        """qc.py ``astype(col_dtypes, errors)``: ``col_dtypes`` is one dtype for every column or a
-        {column label: dtype} mapping.  Only the widening casts of ``DevAstype``; checked here, before any launch,
-        so that a refused cast leaves no half-converted frame."""
-        if errors != "raise":
-            raise NotImplementedError("astype(errors='ignore') is not on the B200 path")
-        return self._astype_map(DevAstype.validate(self.dtypes, col_dtypes))
-
-    def fillna(self, **kwargs):
-        """qc.py:2710-2813: scalar / dict values are a Map; ``method``/``limit`` would be a Fold."""
-        value = kwargs.get("value")
-        if kwargs.get("method") is not None:
-            if kwargs["method"] not in ("ffill", "pad") or value is not None or kwargs.get("limit") is not None \
-                    or kwargs.get("axis") not in (0, "index", None):  # fmt: skip
-                raise NotImplementedError("fillna(method=) on the B200 path: forward fill down the rows, no limit=")
-            return self._ffill(0)
-        if isinstance(value, type(self)):
-            return self.__constructor__(
-                self._modin_frame.n_ary_op(Bound(DevBinary("fillna")), [value._modin_frame], join_type="left")
-            )
-        return self.__constructor__(self._modin_frame.map(Bound(DevFillna(), (), kwargs), dtypes=None))
-
-    # ---- Binary (qc.py:535-624) ---------------------------------------------------------------------
-    add = Binary.register(DevBinary("add"), infer_dtypes="try_sample")
-    radd = Binary.register(DevBinary("radd"), infer_dtypes="try_sample")
-    sub = Binary.register(DevBinary("sub"), infer_dtypes="try_sample")
-    rsub = Binary.register(DevBinary("rsub"), infer_dtypes="try_sample")
-    mul = Binary.register(DevBinary("mul"), infer_dtypes="try_sample")
-    rmul = Binary.register(DevBinary("rmul"), infer_dtypes="try_sample")
-    truediv = Binary.register(DevBinary("truediv"), infer_dtypes="try_sample")
-    rtruediv = Binary.register(DevBinary("rtruediv"), infer_dtypes="try_sample")
-    eq = Binary.register(DevBinary("eq"), infer_dtypes="bool")
-    ne = Binary.register(DevBinary("ne"), infer_dtypes="bool")
-    lt = Binary.register(DevBinary("lt"), infer_dtypes="bool")
-    le = Binary.register(DevBinary("le"), infer_dtypes="bool")
-    gt = Binary.register(DevBinary("gt"), infer_dtypes="bool")
-    ge = Binary.register(DevBinary("ge"), infer_dtypes="bool")
-    # logical ops between bool frames (qc.py:541-571) and ~frame (qc.py `invert`)
-    __and__ = Binary.register(DevLogical("and"), infer_dtypes="bool")
-    __or__ = Binary.register(DevLogical("or"), infer_dtypes="bool")
-    __xor__ = Binary.register(DevLogical("xor"), infer_dtypes="bool")
-    invert = Map.register(DevMap("not"), dtypes=np.bool_)
-
-    # ---- TreeReduce (qc.py:976-1096) ----------------------------------------------------------------
-    count = TreeReduce.register(DevReduce("count"), DevReduce("count", phase="reduce"))
-    sum = TreeReduce.register(DevReduce("sum"), DevReduce("sum", phase="reduce"), compute_dtypes=_dtypes_sum)
-    prod = TreeReduce.register(DevReduce("prod"), DevReduce("prod", phase="reduce"), compute_dtypes=_dtypes_sum)
-    max = TreeReduce.register(DevReduce("max"), DevReduce("max", phase="reduce"))
-    min = TreeReduce.register(DevReduce("min"), DevReduce("min", phase="reduce"))
-    mean = TreeReduce.register(DevMeanMap(), DevMeanReduce(), compute_dtypes=lambda *a, **k: np.dtype("float64"))
-    any = TreeReduce.register(DevBoolReduce("any"), DevBoolReduce("any", phase="reduce"),
-                              compute_dtypes=lambda *a, **k: np.dtype("bool"))  # qc.py:986
-    all = TreeReduce.register(DevBoolReduce("all"), DevBoolReduce("all", phase="reduce"),
-                              compute_dtypes=lambda *a, **k: np.dtype("bool"))  # qc.py:987
-
-    # ---- Reduce (qc.py:1155-1156: std / var = Reduce.register(pandas.DataFrame.std / var)) ---------------------------
-    # qc.py:1101-1102: idxmax / idxmin = Reduce.register(pandas.DataFrame.idxmax / idxmin) -- one arg-reduction pass
-    idxmax = Reduce.register(DevArgReduce("max"))
-    idxmin = Reduce.register(DevArgReduce("min"))
-    _var_frame = Reduce.register(DevVar(sqrt=False))
-    _std_frame = Reduce.register(DevVar(sqrt=True))
-
-    def _var(self, axis=0, skipna=True, ddof=1, numeric_only=False, sqrt=False, **kwargs):
-        """The W variances (standard deviations when ``sqrt``) as a host Series: the API layer of the mirror takes
-        reductions of this kind as W host numbers (identical on every rank)."""
-        qc = (self._std_frame if sqrt else self._var_frame)(axis=axis, skipna=skipna, ddof=ddof, numeric_only=numeric_only)
-        return pandas.Series(qc.to_pandas().iloc[0].to_numpy(dtype=np.float64), index=self.columns, dtype="float64")
+    copy_data = algebra.Map.register(DevMap("copy"), dtypes="copy")
 
     def var(self, axis=0, skipna=True, ddof=1, numeric_only=False, **kwargs):
-        """Reduced result as a host ``pandas.Series`` (W numbers; identical on every rank)."""
-        return self._var(axis, skipna, ddof, numeric_only, sqrt=False)
+        """The W variances as a host ``pandas.Series``: the API layer of the mirror takes reductions of this kind as W
+        host numbers (identical on every rank)."""
+        return self._host_series(super().var(axis=axis, skipna=skipna, ddof=ddof, numeric_only=numeric_only))
 
     def std(self, axis=0, skipna=True, ddof=1, numeric_only=False, **kwargs):
-        return self._var(axis, skipna, ddof, numeric_only, sqrt=True)
+        return self._host_series(super().std(axis=axis, skipna=skipna, ddof=ddof, numeric_only=numeric_only))
 
-    # ---- Fold (qc.py:2429-2431; forward fill is fillna(method="ffill"), qc.py:2809-2810) ----------------------------
-    cumsum = Fold.register(DevCumulative("sum"), shape_preserved=True)
-    cummax = Fold.register(DevCumulative("max"), shape_preserved=True)
-    cummin = Fold.register(DevCumulative("min"), shape_preserved=True)
-    _ffill = Fold.register(DevCumulative("ffill"), shape_preserved=True)
-
-    # ---- GroupByReduce (qc.py:3741-3748; impl table storage_formats/pandas/groupby.py:237-248) ------
-    groupby_sum = GroupByReduce.register(DevGroupbyMap("sum"), DevGroupbyReduce("sum"))
-    groupby_count = GroupByReduce.register(DevGroupbyMap("count"), DevGroupbyReduce("count"))
-    groupby_size = GroupByReduce.register(DevGroupbyMap("size"), DevGroupbyReduce("size"))
-    groupby_mean = GroupByReduce.register(DevGroupbyMap("mean"), DevGroupbyReduce("mean"))
-    groupby_min = GroupByReduce.register(DevGroupbyMap("min"), DevGroupbyReduce("min"))
-    groupby_max = GroupByReduce.register(DevGroupbyMap("max"), DevGroupbyReduce("max"))
-
-    # ---- merge (qc.py:657-667 -> MergeImpl.row_axis_merge merge.py:104-252) --------------------------
-    def merge(self, right, **kwargs):
-        from .merge import row_axis_merge
-
-        return self.__constructor__(row_axis_merge(self, right, _reset_row_index, **kwargs))
-
+    def _host_series(self, qc):
+        return pandas.Series(qc.to_pandas().iloc[0].to_numpy(dtype=np.float64), index=self.columns, dtype="float64")
 
 def group_keys_to_columns(frame):
     """Result frame of a device groupby with ``as_index=False``: keys as leading columns, rows renumbered 0..G-1 over
