@@ -38,8 +38,9 @@ extern "C" {
 #endif
 
 /* 2: round 2 (key statistics, async dense emit, expand / concat / comm entry points); 3: + the Fold template's
- * cumulative scans (mb200_cum_*).  Checked by the binding at load time (modin_b200/_lib.py). */
-#define MB200_ABI_VERSION 3
+ * cumulative scans (mb200_cum_*); 4: + MB200_GB_FIRST / MB200_GB_LAST group tables (row positions, NULL value
+ * columns).  Checked by the binding at load time (modin_b200/_lib.py). */
+#define MB200_ABI_VERSION 4
 #define MB200_MAX_COLS 32 /* max columns per launch == Modin's MinColumnPartitionSize (envvars.py:1149-1190) */
 
 typedef void* mb200_stream_t;
@@ -130,7 +131,11 @@ enum mb200_gb_flags {
   MB200_GB_COUNT = 2, /* cnt[g][v]  += !isnan(x)                                     */
   MB200_GB_SIZE = 4,  /* size[g]    += 1                                             */
   MB200_GB_MIN = 8,   /* acc[g][v]   = min(acc, x)  (NaN skipped; exclusive with SUM / MAX) */
-  MB200_GB_MAX = 16   /* acc[g][v]   = max(acc, x)                                          */
+  MB200_GB_MAX = 16,  /* acc[g][v]   = max(acc, x)                                          */
+  /* row positions (int64) instead of values; each excludes SUM / COUNT / MIN / MAX and the other (SIZE may be set):
+   * see mb200_gb_accumulate and mb200_gb_emit */
+  MB200_GB_FIRST = 32, /* acc[g][v]   = min(position) over the rows whose value in column v is not NaN */
+  MB200_GB_LAST = 64   /* acc[g][v]   = max(position) over the same rows                               */
 };
 
 /* ======================= runtime / memory ================================== */
@@ -249,11 +254,17 @@ int mb200_gb_destroy(mb200_gb_table* table, mb200_stream_t stream);
 /* Hash-aggregate one block: keys[nrows] int64, vals[nvals][nrows] float64 (device).
  * May be called repeatedly (one call per row partition resident on this GPU);
  * replaces GroupByReduce.map alg/groupby.py:124-208 (df.groupby(by).sum() per block).
- * If the table overflows, the call succeeds but mb200_gb_ngroups reports overflow. */
+ * If the table overflows, the call succeeds but mb200_gb_ngroups reports overflow.
+ * FIRST / LAST tables aggregate row POSITIONS: a position counts rows across every mb200_gb_accumulate call on the
+ * table, in call order (the first row of the second call of n1 rows is position n1).  vals[v] may be NULL for them:
+ * the column has no NaN (int64 / bool columns, or any column under skipna=False), every row counts and no value
+ * byte is read.  min / max of positions do not depend on the order of the atomics, so the result is deterministic. */
 int mb200_gb_accumulate(mb200_gb_table* table, const int64_t* keys, const void* const* vals,
                         int64_t nrows, mb200_stream_t stream);
 /* Merge partial tables (keys + partial sums/counts/sizes as produced by mb200_gb_emit) into
- * `table`: replaces GroupByReduce.reduce alg/groupby.py:211-300 (groupby(level=0).sum()). */
+ * `table`: replaces GroupByReduce.reduce alg/groupby.py:211-300 (groupby(level=0).sum()).
+ * Refused for FIRST / LAST tables: positions of one table mean nothing in another; their reduce re-accumulates
+ * the concatenated partial VALUES as raw rows. */
 int mb200_gb_merge_partial(mb200_gb_table* table, const int64_t* keys,
                            const void* const* sums, const void* const* cnts,
                            const int64_t* sizes, int64_t npartial, mb200_stream_t stream);
@@ -263,7 +274,9 @@ int mb200_gb_ngroups(mb200_gb_table* table, int64_t* ngroups, int* overflow,
 /* Scratch bytes needed by mb200_gb_emit for `ngroups` groups. */
 size_t mb200_gb_emit_scratch_bytes(int64_t ngroups);
 /* Write the result block: out_keys[ngroups] (ascending iff sort), out_sums[nvals][ngroups],
- * out_cnts[nvals][ngroups] (int64, may be NULL), out_sizes[ngroups] (may be NULL). */
+ * out_cnts[nvals][ngroups] (int64, may be NULL), out_sizes[ngroups] (may be NULL).
+ * FIRST / LAST tables write int64 positions into out_sums, -1 where the group has no non-NaN value in the column
+ * (mb200_take turns -1 into NaN). */
 int mb200_gb_emit(mb200_gb_table* table, int64_t ngroups, int sort, int64_t* out_keys,
                   void* const* out_sums, void* const* out_cnts, int64_t* out_sizes,
                   void* scratch, mb200_stream_t stream);

@@ -20,7 +20,7 @@ class B200Error(RuntimeError):
     """Raised when a libmodin_b200 call fails (message from mb200_last_error)."""
 
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 # enums (keep in sync with include/modin_b200.h)
 F64, I64, U8 = 0, 1, 2
@@ -40,6 +40,7 @@ PREDICATES = {"isna", "notna", "eq_s", "ne_s", "lt_s", "le_s", "gt_s", "ge_s", "
 RED = {"sum": 0, "min": 1, "max": 2, "count": 3, "prod": 4, "ssd": 5, "argmin": 6, "argmax": 7}
 CUM = {"sum": 0, "max": 1, "min": 2, "ffill": 3}
 GB_SUM, GB_COUNT, GB_SIZE, GB_MIN, GB_MAX = 1, 2, 4, 8, 16
+GB_FIRST, GB_LAST = 32, 64  # int64 row positions instead of values (include/modin_b200.h)
 
 _vp = C.c_void_p
 _vpp = C.POINTER(C.c_void_p)

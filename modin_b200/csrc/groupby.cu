@@ -85,6 +85,7 @@ struct mb200_gb_table {
   // can cover the probe slots AND the accumulators (a stream carries a single window)
   void* arena;
   size_t arena_bytes;
+  long long rows;  // rows accumulated so far: the position of the next accumulate call's first row (FIRST / LAST)
 };
 
 namespace mb200 {
@@ -114,7 +115,10 @@ struct GbParams {
   const long long* keys;
   const void* vals[MB200_MAX_COLS];   // raw values, or partial sums when PARTIAL
   const void* pcnt[MB200_MAX_COLS];   // partial counts (PARTIAL only)
-  const long long* psize;             // partial sizes (PARTIAL only)
+  union {                             // PARTIAL and FIRST / LAST tables exclude each other
+    const long long* psize;           // partial sizes (PARTIAL only)
+    long long row0;                   // FIRST / LAST: table position of row 0 of this launch (earlier calls' rows)
+  };
   long long nrows;
   int dense;              // direct-addressed table: gid = key - kbase
   long long kbase;
@@ -177,9 +181,19 @@ __device__ __forceinline__ void acc_update(const GbParams& p, size_t o, double x
   else if (p.flags & MB200_GB_MAX) red_max_s64(reinterpret_cast<long long*>(p.acc) + o, f64_to_ordered(xv));
 }
 
+// FIRST / LAST (the POS kernels): the accumulator of (group, column) is min / max of the positions of the rows whose
+// value is not NaN -- the same RED.MIN.S64 / RED.MAX.S64 as min / max, on positions instead of ordered values
+__device__ __forceinline__ void pos_update(const GbParams& p, size_t o, long long pos) {
+  if (p.flags & MB200_GB_FIRST) red_min_s64(reinterpret_cast<long long*>(p.acc) + o, pos);
+  else red_max_s64(reinterpret_cast<long long*>(p.acc) + o, pos);
+}
+
 // does adding / min-ing / max-ing / counting `xv` leave a trace in a DENSE table's accumulators?
+// (POS: every non-NaN value moves its position accumulator off the sentinel)
+template <bool POS = false>
 __device__ __forceinline__ bool dense_visible(const GbParams& p, double xv) {
   if (xv != xv) return false;                                                   // NaNs are skipped everywhere
+  if (POS) return true;
   if (p.flags & (MB200_GB_COUNT | MB200_GB_MIN | MB200_GB_MAX)) return true;  // cnt > 0 / acc != sentinel
   return __double_as_longlong(xv) != (long long)0x8000000000000000ULL;          // -0.0 + -0.0 stays -0.0
 }
@@ -327,8 +341,11 @@ __device__ __forceinline__ int resolve_gid(const GbParams& p, long long k, uint6
 }
 
 // ---------------------------------------------------------------- fallback: direct loads
-template <int VARIANT, bool PARTIAL>
+// POS: FIRST / LAST tables (raw rows only) -- positions go to the accumulators, and a NULL value column reads as
+// "no NaN" without a load.  POS = false compiles to the code these kernels had before FIRST / LAST existed.
+template <int VARIANT, bool PARTIAL, bool POS>
 __global__ void __launch_bounds__(kGbThreads, 5) gb_accumulate_kernel(const __grid_constant__ GbParams p) {
+  static_assert(!(POS && PARTIAL), "FIRST / LAST tables take raw rows only");
   __shared__ double s_tile[kGbWarps][8 * kColStride];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const long long nchunks = (p.nrows + 31) >> 5;
@@ -347,7 +364,8 @@ __global__ void __launch_bounds__(kGbThreads, 5) gb_accumulate_kernel(const __gr
       const int nc = p.nvals < 8 ? p.nvals : 8;
 #pragma unroll
       for (int c = 0; c < 8; ++c)
-        x[c] = (c < nc && valid) ? ldg_stream_f64(static_cast<const double*>(p.vals[c]) + row, pol) : 0.0;
+        x[c] = (c < nc && valid && (!POS || p.vals[c])) ? ldg_stream_f64(static_cast<const double*>(p.vals[c]) + row, pol)
+                                                        : 0.0;
     }
     {
       // rows past the end borrow lane 0's key (lane 0 is always valid in a live chunk) so that they join
@@ -366,7 +384,9 @@ __global__ void __launch_bounds__(kGbThreads, 5) gb_accumulate_kernel(const __gr
       if (c0 > 0) {
 #pragma unroll
         for (int c = 0; c < 8; ++c)
-          x[c] = (c < nc && valid) ? ldg_stream_f64(static_cast<const double*>(p.vals[c0 + c]) + row, pol) : 0.0;
+          x[c] = (c < nc && valid && (!POS || p.vals[c0 + c]))
+                     ? ldg_stream_f64(static_cast<const double*>(p.vals[c0 + c]) + row, pol)
+                     : 0.0;
       }
       if (VARIANT == 1) {  // lane == row (kept for measurement)
         bool rowvis = false;
@@ -374,8 +394,12 @@ __global__ void __launch_bounds__(kGbThreads, 5) gb_accumulate_kernel(const __gr
         for (int c = 0; c < 8; ++c) {
           if (c < nc && live) {
             const size_t o = (size_t)gid * p.vstride + c0 + c;
-            rowvis = rowvis || (!PARTIAL && dense_visible(p, x[c]));
-            if (x[c] == x[c]) acc_update(p, o, x[c], keep);
+            rowvis = rowvis || (!PARTIAL && dense_visible<POS>(p, x[c]));
+            if (POS) {
+              if (x[c] == x[c]) pos_update(p, o, p.row0 + row);
+            } else if (x[c] == x[c]) {
+              acc_update(p, o, x[c], keep);
+            }
             if (p.flags & MB200_GB_COUNT) {
               if (PARTIAL) red_add_u64(p.cnt + o, static_cast<const long long*>(p.pcnt[c0 + c])[row], keep);
               else if (x[c] == x[c]) red_add_u64(p.cnt + o, 1LL, keep);
@@ -401,8 +425,12 @@ __global__ void __launch_bounds__(kGbThreads, 5) gb_accumulate_kernel(const __gr
           if ((base + r < p.nrows) && g < gcap) rowok |= 1u << kk;
           if (ok) {
             const size_t o = (size_t)g * p.vstride + c0 + c;
-            if (!PARTIAL && dense_visible(p, xv)) seen |= 1u << kk;
-            if (xv == xv) acc_update(p, o, xv, keep);
+            if (!PARTIAL && dense_visible<POS>(p, xv)) seen |= 1u << kk;
+            if (POS) {
+              if (xv == xv) pos_update(p, o, p.row0 + base + r);
+            } else if (xv == xv) {
+              acc_update(p, o, xv, keep);
+            }
             if (p.flags & MB200_GB_COUNT) {
               if (PARTIAL) red_add_u64(p.cnt + o, static_cast<const long long*>(p.pcnt[c0 + c])[base + r], keep);
               else if (xv == xv) red_add_u64(p.cnt + o, 1LL, keep);
@@ -447,9 +475,10 @@ constexpr int kHotBytesSum = kHotSlots * 4 + kHotSlots * kHotStride * 8;        
 constexpr int kHotBytes = kHotBytesSum + kHotSlots * kHotStride * 4;                     // ... + counts
 constexpr int kHotBit = 1 << 30;  // group ids are < 2^29
 
-template <bool HOT, int STAGES>
+template <bool HOT, int STAGES, bool POS>
 __global__ void __launch_bounds__(kGbTmaThreads) gb_accumulate_tma_kernel(const __grid_constant__ GbParams p,
                                                                           long long ntiles) {
+  static_assert(!(HOT && POS), "FIRST / LAST tables do not take the hot-group cache");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + STAGES * kStageBytes);
   uint64_t* empty = full + STAGES;
@@ -483,16 +512,20 @@ __global__ void __launch_bounds__(kGbTmaThreads) gb_accumulate_tma_kernel(const 
     // ---------------- producer: (1 + nv) bulk copies of 2 KiB per tile
     if (lane == 0) {
       const uint64_t pol = l2_policy_evict_first();
+      int ncopy = nv;  // POS: NULL value columns ("no NaN") are not copied
+      if (POS)
+        for (int c = 0; c < nv; ++c) ncopy -= p.vals[c] ? 0 : 1;
       for (long long k = 0; k < nmine; ++k) {
         const int s = (int)(k % STAGES);
         if (k >= STAGES) mbar_wait(&empty[s], (uint32_t)(((k / STAGES) - 1) & 1));
         const long long row0 = (first + k * gridDim.x) * kTileRows;
         double* stage = reinterpret_cast<double*>(smem_raw + (size_t)s * kStageBytes);
-        mbar_expect_tx(&full[s], (uint32_t)((1 + nv) * kTileRows * 8));
+        mbar_expect_tx(&full[s], (uint32_t)((1 + ncopy) * kTileRows * 8));
         tma_bulk_g2s(stage, p.keys + row0, kTileRows * 8, &full[s], pol);
         for (int c = 0; c < nv; ++c)
-          tma_bulk_g2s(stage + (size_t)(1 + c) * kTileColStride, static_cast<const double*>(p.vals[c]) + row0,
-                       kTileRows * 8, &full[s], pol);
+          if (!POS || p.vals[c])
+            tma_bulk_g2s(stage + (size_t)(1 + c) * kTileColStride, static_cast<const double*>(p.vals[c]) + row0,
+                         kTileRows * 8, &full[s], pol);
       }
     }
     return;
@@ -500,6 +533,7 @@ __global__ void __launch_bounds__(kGbTmaThreads) gb_accumulate_tma_kernel(const 
   // ---------------- consumers: warp w owns rows [32w, 32w + 32) of every tile
   const uint64_t keep = table_policy(p.policy_mode);
   const int c = lane & 7;
+  const bool nullcol = POS && c < nv && !p.vals[c];  // POS: this lane's column has no NaN and no staged tile
   for (long long k = 0; k < nmine; ++k) {
     const int s = (int)(k % STAGES);
     mbar_wait(&full[s], (uint32_t)((k / STAGES) & 1));
@@ -536,9 +570,11 @@ __global__ void __launch_bounds__(kGbTmaThreads) gb_accumulate_tma_kernel(const 
       const int g = HOT ? (pg & ~kHotBit) : pg;
       gs[kk] = g;
       if (c < nv && g < gcap) {
-        const double xv = vt[c * kTileColStride + r];
-        if (dense_visible(p, xv)) seen |= 1u << kk;
-        if (xv == xv) {
+        const double xv = nullcol ? 0.0 : vt[c * kTileColStride + r];
+        if (dense_visible<POS>(p, xv)) seen |= 1u << kk;
+        if (POS) {
+          if (xv == xv) pos_update(p, (size_t)g * p.vstride + c, p.row0 + (first + k * gridDim.x) * kTileRows + warp * 32 + r);
+        } else if (xv == xv) {
           if (HOT && (pg & kHotBit)) {
             const int o = (g & (kHotSlots - 1)) * kHotStride + c;
             if (p.flags & MB200_GB_SUM) atomicAdd(&s_hot[o], xv);
@@ -602,6 +638,9 @@ struct SmemTableLayout {
   int zstride;  // replica stride of the size array (odd)
 };
 
+// POS: FIRST / LAST tables -- the MIN / MAX code on row positions (FIRST = min, LAST = max), NULL value columns read
+// as "no NaN" without a load.
+template <bool POS>
 __global__ void __launch_bounds__(kSmemThreads, 1) gb_accumulate_smem_kernel(const __grid_constant__ GbParams p,
                                                                              const SmemTableLayout lay) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -614,7 +653,8 @@ __global__ void __launch_bounds__(kSmemThreads, 1) gb_accumulate_smem_kernel(con
   const int nv = p.nvals, vs = p.vstride, svs = lay.svs;
   const int R = (int)p.gcap;
   const int nrep = lay.nrep, rstride = lay.rstride, zstride = lay.zstride;
-  const bool f_sum = p.flags & MB200_GB_SUM, f_min = p.flags & MB200_GB_MIN, f_max = p.flags & MB200_GB_MAX;
+  const bool f_sum = !POS && (p.flags & MB200_GB_SUM);
+  const bool f_min = p.flags & (POS ? MB200_GB_FIRST : MB200_GB_MIN), f_max = p.flags & (POS ? MB200_GB_LAST : MB200_GB_MAX);
   const bool f_cnt = p.flags & MB200_GB_COUNT, f_size = p.flags & MB200_GB_SIZE;
   const bool has_acc = f_sum || f_min || f_max;
   const long long init = f_min ? 0x7fffffffffffffffLL : (f_max ? (long long)0x8000000000000000ULL : 0LL);
@@ -637,7 +677,7 @@ __global__ void __launch_bounds__(kSmemThreads, 1) gb_accumulate_smem_kernel(con
       const int nc = nv < 8 ? nv : 8;
 #pragma unroll
       for (int c = 0; c < 8; ++c)
-        x[c] = (c < nc) ? ldg_stream_f64(static_cast<const double*>(p.vals[c]) + row, pol) : 0.0;
+        x[c] = (c < nc && (!POS || p.vals[c])) ? ldg_stream_f64(static_cast<const double*>(p.vals[c]) + row, pol) : 0.0;
     }
     const unsigned long long d = (unsigned long long)key - (unsigned long long)p.kbase;
     if (d >= (unsigned long long)R) {
@@ -652,15 +692,16 @@ __global__ void __launch_bounds__(kSmemThreads, 1) gb_accumulate_smem_kernel(con
       if (c0 > 0) {
 #pragma unroll
         for (int c = 0; c < 8; ++c)
-          x[c] = (c < nc) ? ldg_stream_f64(static_cast<const double*>(p.vals[c0 + c]) + row, pol) : 0.0;
+          x[c] = (c < nc && (!POS || p.vals[c0 + c])) ? ldg_stream_f64(static_cast<const double*>(p.vals[c0 + c]) + row, pol)
+                                                      : 0.0;
       }
 #pragma unroll
       for (int c = 0; c < 8; ++c) {
         if (c < nc && x[c] == x[c]) {
           const int o = rbase + gid * svs + c0 + c;
           if (f_sum) atomicAdd(&s_acc[o], x[c]);
-          else if (f_min) atomicMin(&s_acc_i[o], f64_to_ordered(x[c]));
-          else if (f_max) atomicMax(&s_acc_i[o], f64_to_ordered(x[c]));
+          else if (f_min) atomicMin(&s_acc_i[o], POS ? p.row0 + row : f64_to_ordered(x[c]));
+          else if (f_max) atomicMax(&s_acc_i[o], POS ? p.row0 + row : f64_to_ordered(x[c]));
           if (f_cnt) atomicAdd(&s_cnt[o], 1u);
         }
       }
@@ -790,7 +831,11 @@ __global__ void gb_emit_kernel(const __grid_constant__ EmitParams p) {
   for (int v = 0; v < p.nvals; ++v) {
     if (p.out_sums[v] && p.acc) {
       double val = p.acc[(size_t)g * p.vstride + v];
-      if (p.flags & (MB200_GB_MIN | MB200_GB_MAX)) {
+      if (p.flags & (MB200_GB_FIRST | MB200_GB_LAST)) {  // int64 position; -1: no non-NaN value in the group
+        const long long o = __double_as_longlong(val);
+        const bool empty = (p.flags & MB200_GB_FIRST) ? (o == 0x7fffffffffffffffLL) : (o == (long long)0x8000000000000000ULL);
+        val = __longlong_as_double(empty ? -1LL : o);
+      } else if (p.flags & (MB200_GB_MIN | MB200_GB_MAX)) {
         const long long o = __double_as_longlong(val);
         const bool empty = (p.flags & MB200_GB_MIN) ? (o == 0x7fffffffffffffffLL) : (o == (long long)0x8000000000000000ULL);
         val = empty ? __longlong_as_double(0x7ff8000000000000LL) : ordered_to_f64(o);
@@ -968,15 +1013,15 @@ static int gb_variant_from_env(size_t table_bytes, size_t l2_bytes) {
   return 0;
 }
 
-template <int VARIANT, bool PARTIAL>
+template <int VARIANT, bool PARTIAL, bool POS = false>
 static int launch_ldg(const GbParams& p, const DevProps& dp, cudaStream_t st) {
   int occ = 0;
-  MB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, gb_accumulate_kernel<VARIANT, PARTIAL>, kGbThreads, 0));
+  MB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, gb_accumulate_kernel<VARIANT, PARTIAL, POS>, kGbThreads, 0));
   const long long nchunks = (p.nrows + 31) / 32;
   long long grid = (long long)dp.sm_count * (occ < 1 ? 1 : occ);
   const long long need = (nchunks + kGbWarps - 1) / kGbWarps;
   if (grid > need) grid = need;
-  gb_accumulate_kernel<VARIANT, PARTIAL><<<(unsigned)grid, kGbThreads, 0, st>>>(p);
+  gb_accumulate_kernel<VARIANT, PARTIAL, POS><<<(unsigned)grid, kGbThreads, 0, st>>>(p);
   MB_LAUNCH_CHECK("gb_accumulate_kernel");
   return 0;
 }
@@ -1003,16 +1048,19 @@ static int gb_launch(mb200_gb_table* t, const long long* keys, const void* const
   p.kbase = t->kbase;
   p.present = t->present;
   p.keys = keys;
+  const bool pos = t->flags & (MB200_GB_FIRST | MB200_GB_LAST);
+  if (pos && partial) return fail("groupby", "FIRST / LAST tables do not merge partial tables");
   bool aligned = aligned16(keys);
   for (int c = 0; c < t->nvals; ++c) {
     p.vals[c] = vals ? vals[c] : nullptr;
     p.pcnt[c] = pcnt ? pcnt[c] : nullptr;
     if ((t->flags & (MB200_GB_SUM | MB200_GB_COUNT | MB200_GB_MIN | MB200_GB_MAX)) && !p.vals[c])
-      return fail("groupby", "null value column");
+      return fail("groupby", "null value column");  // FIRST / LAST: NULL = a column without NaN
     if (partial && (t->flags & MB200_GB_COUNT) && !p.pcnt[c]) return fail("groupby", "null partial count column");
     aligned = aligned && aligned16(p.vals[c]);
   }
-  p.psize = psize;
+  if (pos) p.row0 = t->rows;
+  else p.psize = psize;
   if (partial && (t->flags & MB200_GB_SIZE) && !psize) return fail("groupby", "null partial size column");
   p.nrows = nrows;
   {
@@ -1022,7 +1070,7 @@ static int gb_launch(mb200_gb_table* t, const long long* keys, const void* const
     p.prefetch = (pf && pf[0] == '1') ? 1 : 0;
   }
   const size_t table_bytes = (size_t)t->cap * sizeof(Slot) + (size_t)t->gcap * t->vstride * 8 *
-                                                                  (((t->flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX)) ? 1 : 0) +
+                                                                  (((t->flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST)) ? 1 : 0) +
                                                                    ((t->flags & MB200_GB_COUNT) ? 1 : 0));
   const int variant = gb_variant_from_env(table_bytes, dp.l2_bytes);
 
@@ -1094,7 +1142,7 @@ static int gb_launch(mb200_gb_table* t, const long long* keys, const void* const
       off = 0;
       lay.nrep = nrep;
       lay.acc_off = (unsigned)off;
-      if (t->flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX)) off += elems * 8;
+      if (t->flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST)) off += elems * 8;
       lay.cnt_off = (unsigned)off;
       if (t->flags & MB200_GB_COUNT) off += (elems * 4 + 15) & ~(size_t)15;
       lay.size_off = (unsigned)off;
@@ -1105,18 +1153,19 @@ static int gb_launch(mb200_gb_table* t, const long long* keys, const void* const
       if (off <= dp.smem_optin) break;
     }
     if (!(e && e[0] == '0') && off <= dp.smem_optin) {
-      MB_CUDA(cudaFuncSetAttribute(gb_accumulate_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)off));
+      auto kern = pos ? gb_accumulate_smem_kernel<true> : gb_accumulate_smem_kernel<false>;
+      MB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)off));
       long long grid = dp.sm_count;
       const long long need = (nrows + kSmemThreads - 1) / kSmemThreads;
       if (grid > need) grid = need;
-      gb_accumulate_smem_kernel<<<(unsigned)grid, kSmemThreads, off, st>>>(p, lay);
+      kern<<<(unsigned)grid, kSmemThreads, off, st>>>(p, lay);
       MB_LAUNCH_CHECK("gb_accumulate_smem_kernel");
       return 0;
     }
   }
   if (variant == 0 && !partial && aligned && t->nvals <= 8 && nrows >= kTileRows) {
     const long long ntiles = nrows / kTileRows;
-    const bool hot = t->skewed && !(t->flags & (MB200_GB_MIN | MB200_GB_MAX | MB200_GB_SIZE));
+    const bool hot = t->skewed && !(t->flags & (MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST | MB200_GB_SIZE));
     // hashed tables: a 2-stage ring lets 5 CTAs share an SM instead of 4 (the probe chain wants warps, not staging
     // depth); MB200_GB_STAGES=3 restores the 3-stage ring for comparison
     const char* se = getenv("MB200_GB_STAGES");
@@ -1124,9 +1173,10 @@ static int gb_launch(mb200_gb_table* t, const long long* keys, const void* const
     const size_t smem = hot   ? (size_t)hot_offset(kHotStages) + ((t->flags & MB200_GB_COUNT) ? kHotBytes : kHotBytesSum)
                         : two ? (size_t)2 * kStageBytes + 2 * 2 * sizeof(uint64_t)
                               : (size_t)kGbStages * kStageBytes + 2 * kGbStages * sizeof(uint64_t);
-    auto kern = hot   ? gb_accumulate_tma_kernel<true, kHotStages>
-                : two ? gb_accumulate_tma_kernel<false, 2>
-                      : gb_accumulate_tma_kernel<false, kGbStages>;
+    auto kern = hot   ? gb_accumulate_tma_kernel<true, kHotStages, false>
+                : pos ? (two ? gb_accumulate_tma_kernel<false, 2, true> : gb_accumulate_tma_kernel<false, kGbStages, true>)
+                : two ? gb_accumulate_tma_kernel<false, 2, false>
+                      : gb_accumulate_tma_kernel<false, kGbStages, false>;
     MB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
     MB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kGbTmaThreads, smem));
@@ -1140,12 +1190,15 @@ static int gb_launch(mb200_gb_table* t, const long long* keys, const void* const
     p.keys = keys + done;
     for (int c = 0; c < t->nvals; ++c)
       if (p.vals[c]) p.vals[c] = static_cast<const double*>(p.vals[c]) + done;
+    p.row0 += done;
     p.nrows = nrows - done;
   }
   if (variant == 2) {
+    if (pos) return launch_ldg<1, false, true>(p, dp, st);
     if (partial) return launch_ldg<1, true>(p, dp, st);
     return launch_ldg<1, false>(p, dp, st);
   }
+  if (pos) return launch_ldg<0, false, true>(p, dp, st);
   if (partial) return launch_ldg<0, true>(p, dp, st);
   return launch_ldg<0, false>(p, dp, st);
 }
@@ -1176,7 +1229,7 @@ extern "C" int mb200_gb_create_dense(mb200_gb_table** table, int64_t key_min, in
   if (range == 0 || range > (1ULL << 29)) return fail("mb200_gb_create_dense", "key range above 2^29");
   DenseArrays ext{acc, cnt, size, present};
   if (present) {
-    const bool need_acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX);
+    const bool need_acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST);
     if ((need_acc && !acc) || ((flags & MB200_GB_COUNT) && !cnt) || ((flags & MB200_GB_SIZE) && !size))
       return fail("mb200_gb_create_dense", "caller-owned arrays: every array the flags need must be given");
     if (!aligned16(acc) || !aligned16(cnt) || !aligned16(size) || !aligned16(present))
@@ -1199,7 +1252,7 @@ extern "C" int mb200_gb_adopt_dense(mb200_gb_table** table, int64_t key_min, int
   if (key_max < key_min) return fail("mb200_gb_adopt_dense", "empty key range");
   const unsigned long long range = (unsigned long long)key_max - (unsigned long long)key_min + 1ULL;
   if (range == 0 || range > (1ULL << 29)) return fail("mb200_gb_adopt_dense", "key range above 2^29");
-  const bool need_acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX);
+  const bool need_acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST);
   if (!present || (need_acc && !acc) || ((flags & MB200_GB_COUNT) && !cnt) || ((flags & MB200_GB_SIZE) && !size))
     return fail("mb200_gb_adopt_dense", "every array the flags need must be given");
   if (!aligned16(acc) || !aligned16(cnt) || !aligned16(size) || !aligned16(present))
@@ -1255,6 +1308,10 @@ static int gb_create_impl(mb200_gb_table** table, int64_t group_capacity, int nv
   if (nvals < 0 || nvals > MB200_MAX_COLS) return fail("mb200_gb_create", "nvals out of range (0..32)");
   if (group_capacity < 1) group_capacity = 1;
   if (group_capacity > (1LL << 29)) return fail("mb200_gb_create", "group capacity above 2^29");
+  if ((flags & (MB200_GB_FIRST | MB200_GB_LAST)) &&
+      (flags & (MB200_GB_SUM | MB200_GB_COUNT | MB200_GB_MIN | MB200_GB_MAX) ||
+       (flags & (MB200_GB_FIRST | MB200_GB_LAST)) == (MB200_GB_FIRST | MB200_GB_LAST)))
+    return fail("mb200_gb_create", "FIRST / LAST exclude every other accumulator flag");
   DevProps dp;
   if (int rc = dev_props(&dp)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
@@ -1292,7 +1349,7 @@ static int gb_create_impl(mb200_gb_table** table, int64_t group_capacity, int nv
   } else {
     const size_t slot_b = ((size_t)t->cap * sizeof(Slot) + 255) & ~(size_t)255;
     const size_t acc_b = (accb + 255) & ~(size_t)255;
-    const bool has_acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX);
+    const bool has_acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST);
     const size_t size_b = (((size_t)t->gcap * 8) + 255) & ~(size_t)255;
     t->arena_bytes = slot_b + (has_acc ? acc_b : 0) + ((flags & MB200_GB_COUNT) ? acc_b : 0) +
                      ((flags & MB200_GB_SIZE) ? size_b : 0);
@@ -1323,13 +1380,14 @@ static int gb_create_impl(mb200_gb_table** table, int64_t group_capacity, int nv
     } else {
       MB_TRY(cudaMemsetAsync(t->acc, 0, accb, st));
     }
-  } else if (flags & (MB200_GB_MIN | MB200_GB_MAX)) {
+  } else if (flags & (MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST)) {
     if (!t->borrowed && dense) MB_TRY(cudaMallocAsync((void**)&t->acc, accb, st));
     // "no value yet": INT64_MAX = bytes ff..ff 7f for min is not a byte pattern; use the fill kernel
     gb_fill_kernel<<<(unsigned)dp.sm_count * 4, 256, 0, st>>>(reinterpret_cast<long long*>(t->acc),
                                                              (long long)(accb / 8),
-                                                             (flags & MB200_GB_MIN) ? 0x7fffffffffffffffLL
-                                                                                    : (long long)0x8000000000000000ULL);
+                                                             (flags & (MB200_GB_MIN | MB200_GB_FIRST))
+                                                                 ? 0x7fffffffffffffffLL
+                                                                 : (long long)0x8000000000000000ULL);
     MB_TRY(cudaGetLastError());
     g_launches.fetch_add(1);
   }
@@ -1384,8 +1442,11 @@ extern "C" int mb200_gb_accumulate(mb200_gb_table* t, const int64_t* keys, const
   if (!t) return fail("mb200_gb_accumulate", "null table");
   if (nrows < 0) return fail("mb200_gb_accumulate", "negative nrows");
   if (nrows > 0 && !keys) return fail("mb200_gb_accumulate", "null keys");
-  return gb_launch(t, reinterpret_cast<const long long*>(keys), vals, nullptr, nullptr, nrows, false,
-                   (cudaStream_t)stream);
+  if (int rc = gb_launch(t, reinterpret_cast<const long long*>(keys), vals, nullptr, nullptr, nrows, false,
+                         (cudaStream_t)stream))
+    return rc;
+  t->rows += nrows;
+  return 0;
 }
 
 extern "C" int mb200_gb_merge_partial(mb200_gb_table* t, const int64_t* keys, const void* const* sums,
@@ -1402,7 +1463,7 @@ static int dense_finalize_presence(mb200_gb_table* t, cudaStream_t st) {
   const long long n = t->win_hi - t->win_lo;
   if (n <= 0) return 0;
   const long long init = (t->flags & MB200_GB_SUM)   ? (long long)0x8000000000000000ULL
-                         : (t->flags & MB200_GB_MIN) ? 0x7fffffffffffffffLL
+                         : (t->flags & (MB200_GB_MIN | MB200_GB_FIRST)) ? 0x7fffffffffffffffLL
                                                      : (long long)0x8000000000000000ULL;
   dense_presence_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
       reinterpret_cast<unsigned char*>(t->present), reinterpret_cast<const long long*>(t->acc), t->cnt, t->size,

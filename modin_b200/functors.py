@@ -1276,7 +1276,12 @@ _PARTIALS = {
     "count": _Partial(_lib.GB_COUNT, ("cnts",)),
     "size": _Partial(_lib.GB_SIZE, ("sizes",)),
     "mean": _Partial(_lib.GB_SUM | _lib.GB_COUNT, ("sums", "cnts")),  # mean = sums / counts, in _finished_block
+    # the partial of first / last holds the VALUES, in their own dtypes (``_first_last``); the table behind it holds
+    # row positions, so partials are never merged as tables (no ``merge_partial``)
+    "first": _Partial(_lib.GB_FIRST, ("sums",)),
+    "last": _Partial(_lib.GB_LAST, ("sums",)),
 }
+_POSITION_AGGS = ("first", "last")
 
 
 def _partial_cols(agg, sums, cnts, sizes):
@@ -1362,19 +1367,47 @@ def _finished_block(agg, keys, key_label, cols, labels):
     return _group_block(cols, _partial_labels(agg, labels), keys, key_label)
 
 
+def _first_last(agg, key: DeviceColumn, vals, skipna: bool, capacity_hint: int):
+    """``groupby.first`` / ``last`` of the value columns ``vals`` (any dtype) by ``key``: the ascending group keys and
+    one column per value column, in its own dtype -- a gather of the row each group takes from it.
+
+    One FIRST / LAST table gives every group the min / max row position over the non-NaN values of a slot.  Under
+    ``skipna`` each float64 column has a slot of its own; every column that cannot hold NaN (int64, bool) and every
+    column under ``skipna=False`` shares ONE slot without values (a NULL column: the group's first / last row).  A
+    float64 group without a non-NaN value gets position -1, which the gather turns into NaN."""
+    slots, slot_of, shared = [], [], None
+    for v in vals:
+        if skipna and v.dtype == np.float64:
+            slot_of.append(len(slots))
+            slots.append(v)
+        else:
+            if shared is None:
+                shared = len(slots)
+                slots.append(None)
+            slot_of.append(shared)
+    flags = _lib.GB_FIRST if agg == "first" else _lib.GB_LAST
+    keys, pos, _, _ = ops.hash_aggregate([(key, slots)], flags, capacity_hint)
+    return keys, [ops.take_columns([v], pos[s])[0] for v, s in zip(vals, slot_of)]
+
+
 class DevGroupbyMap(DevFn):
     """GroupByReduce.map (alg/groupby.py:124-208): hash-aggregate one row block against its
-    slice of `by` into a partial table (index = keys, ascending)."""
+    slice of `by` into a partial table (index = keys, ascending).  ``skipna``: first / last only."""
 
-    def __init__(self, agg: str, capacity_hint: int = 1 << 20):
+    def __init__(self, agg: str, capacity_hint: int = 1 << 20, skipna: bool = True):
         if agg not in _PARTIALS:
             raise NotImplementedError(f"groupby.{agg} is not on the B200 path")
         self.agg = agg
         self.op = f"groupby_{agg}_map"
         self.capacity_hint = capacity_hint
+        self.skipna = skipna
 
     def __call__(self, block, by_block=None, *args, **kwargs):
         key, key_label, vals, labels = _split_key_values(block, by_block, self.op)
+        if self.agg in _POSITION_AGGS:
+            # the partial is what pandas' groupby.first / last gives for this row block
+            keys, cols = _first_last(self.agg, key, vals, self.skipna, self.capacity_hint)
+            return _group_block(cols, labels, keys, key_label)
         vals = _aggregated_values(self.agg, vals)
         keys, sums, cnts, sizes = ops.hash_aggregate([(key, vals)], _PARTIALS[self.agg].flags, self.capacity_hint)
         return _group_block(_partial_cols(self.agg, sums, cnts, sizes), _partial_labels(self.agg, labels), keys, key_label)
@@ -1396,15 +1429,24 @@ def keys_to_columns(block: DeviceBlock, offset: int = 0) -> DeviceBlock:
 
 class DevGroupbyReduce(DevFn):
     """GroupByReduce.reduce (alg/groupby.py:211-300): regroup the concatenated partial tables by
-    key (level 0) with the reduce aggregation (sum of sums / counts / sizes; mean = sum/count)."""
+    key (level 0) with the reduce aggregation (sum of sums / counts / sizes; mean = sum/count).
 
-    def __init__(self, agg: str):
+    first / last regroup the partial VALUES as raw rows (``_first_last`` again): the first of the per-partition
+    firsts, taken in row order, is the first.  That rests on two orders -- the partials of a rank's row partitions
+    are concatenated in partition order (``map_axis_partitions``), and ``dist.exchange_by_key_range`` concatenates
+    what the ranks send in rank order -- and on a NaN partial meaning "no value in that partition", exactly as a NaN
+    row does (under ``skipna=False`` every column takes the group's first / last partial row)."""
+
+    def __init__(self, agg: str, skipna: bool = True):
         self.agg = agg
         self.op = f"groupby_{agg}_reduce"
+        self.skipna = skipna
 
     def _merge(self, keys, cols):
         """Regroup partial rows by key -> ascending unique keys + merged partial columns (same layout as the input).
         Partial sums add up, partial minima / maxima reduce with min / max, counts and sizes add up."""
+        if self.agg in _POSITION_AGGS:
+            return _first_last(self.agg, keys, list(cols), self.skipna, len(keys))
         layout = _PARTIALS[self.agg]
         W = len(cols) // len(layout.arrays)
         got = {name: list(cols[i * W : (i + 1) * W]) for i, name in enumerate(layout.arrays)}
@@ -1437,10 +1479,12 @@ class DevGroupbyReduce(DevFn):
         range, ascending -- the concatenation over ranks is the reference's key-sorted result."""
         from . import dist
 
-        rk, rcols = dist.exchange_by_key_range(k.data, [c.data for c in cols])
+        bools = [c.dtype == np.bool_ for c in cols]  # first / last: the exchange moves 8-byte columns, so int64 0 / 1
+        rk, rcols = dist.exchange_by_key_range(k.data, [c.data for c in ops.cast_columns_i64(cols)])
         rkeys = DeviceColumn(rk, np.int64)
-        rc = [DeviceColumn(t_, c.dtype) for t_, c in zip(rcols, cols)]
-        return self._merge(rkeys, rc) if len(rkeys) else (rkeys, rc)
+        rc = [DeviceColumn(t_, np.dtype(np.int64) if b else c.dtype) for t_, c, b in zip(rcols, cols, bools)]
+        k, rc = self._merge(rkeys, rc) if len(rkeys) else (rkeys, rc)
+        return k, [ops.map_columns("ne_s", [c], s0=[0])[0] if b else c for c, b in zip(rc, bools)]
 
 
 def fused_dense_groupby(map_fn: "DevGroupbyMap", reduce_fn: "DevGroupbyReduce", blocks, by_blocks):
@@ -1457,6 +1501,10 @@ def fused_dense_groupby(map_fn: "DevGroupbyMap", reduce_fn: "DevGroupbyReduce", 
 
     agg = map_fn.agg
     if agg != reduce_fn.agg or not blocks or len(blocks) != len(by_blocks):
+        return None
+    if agg in _POSITION_AGGS:
+        # merging position tables across GPUs would need the values gathered across GPUs too: the general path
+        # (still one dense table per partition when the key range allows) does first / last
         return None
     inputs = [_split_key_values(block, by_block, map_fn.op) for block, by_block in zip(blocks, by_blocks)]
     key_label, labels = inputs[0][1], (inputs[0][3] if agg != "size" else inputs[0][3][:0])

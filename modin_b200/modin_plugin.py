@@ -438,6 +438,8 @@ def register(shims: bool | None = None):
         groupby_mean = _by_level(Ops.groupby_mean)
         groupby_min = _by_level(Ops.groupby_min)
         groupby_max = _by_level(Ops.groupby_max)
+        # first / last come from the shared definition as they are; it asks this for the key of groupby(level=)
+        _b200_level_key = _labels_as_by
 
         def unique(self, keep="first", ignore_index=True, subset=None):
             """qc.py:2231-2270 -- what ``drop_duplicates`` (modin/pandas/base.py:1600-1623) and ``Series.unique``

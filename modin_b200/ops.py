@@ -255,7 +255,8 @@ def arg_reduce_columns(op: str, cols: Sequence[DeviceColumn], variant: int = 0):
 
 
 # ------------------------------------------------------------------ GroupByReduce
-_GB_ACC = _lib.GB_SUM | _lib.GB_MIN | _lib.GB_MAX
+_GB_POS = _lib.GB_FIRST | _lib.GB_LAST  # tables of int64 row positions (first / last)
+_GB_ACC = _lib.GB_SUM | _lib.GB_MIN | _lib.GB_MAX | _GB_POS
 _DENSE_ARRAYS = ("acc", "cnt", "size", "present")
 
 
@@ -323,7 +324,7 @@ class GroupTable:
 
     def collective_arrays(self):
         """(tensor, reduce-op, elements per key) triples whose element-wise reduction over ranks merges dense tables."""
-        acc_op = "sum" if self.flags & _lib.GB_SUM else ("min" if self.flags & _lib.GB_MIN else "max")
+        acc_op = "sum" if self.flags & _lib.GB_SUM else ("min" if self.flags & (_lib.GB_MIN | _lib.GB_FIRST) else "max")
         vs = value_stride(self.nvals)
         out = [(self.acc, acc_op, vs), (self.cnt, "sum", vs), (self.size, "sum", 1), (self.present, "max", 1)]
         return [(x, op, per) for x, op, per in out if x is not None]
@@ -351,13 +352,17 @@ class GroupTable:
         """Skewed keys: accumulate with the per-CTA hot-group cache (mb200_gb_hint_skew)."""
         _lib.check(self.lib.mb200_gb_hint_skew(self.handle, 1 if skewed else 0))
 
-    def accumulate(self, keys: DeviceColumn, vals: Sequence[DeviceColumn]):
+    def accumulate(self, keys: DeviceColumn, vals: Sequence[Optional[DeviceColumn]]):
+        """Aggregate rows ``keys`` / ``vals`` (float64 columns).  A first / last table also takes None for a column
+        without NaN: every row of it counts.  Positions run on across calls, in call order."""
         if keys.dtype != np.int64:
             raise TypeError("device groupby needs an int64 key column")
         for v in vals:
-            if v.dtype != np.float64:
+            if v is None and self.flags & _GB_POS:
+                continue
+            if v is None or v.dtype != np.float64:
                 raise TypeError("device groupby aggregates float64 value columns")
-        ptrs = _lib.ptr_array([v.ptr for v in vals])
+        ptrs = _lib.ptr_array([v.ptr if v is not None else None for v in vals])
         with _timed("gb_accumulate"):
             _lib.check(self.lib.mb200_gb_accumulate(self.handle, keys.ptr, ptrs, len(keys), current_stream()))
 
@@ -377,7 +382,8 @@ class GroupTable:
 
     def _outputs(self, rows: int):
         """Empty (keys, sums, cnts, sizes) columns of ``rows`` rows for what this table emits."""
-        sums = [DeviceColumn.empty(rows, np.float64) for _ in range(self.nvals)] if self.flags & _GB_ACC else None
+        acc_dtype = np.int64 if self.flags & _GB_POS else np.float64  # first / last emit row positions
+        sums = [DeviceColumn.empty(rows, acc_dtype) for _ in range(self.nvals)] if self.flags & _GB_ACC else None
         cnts = [DeviceColumn.empty(rows, np.int64) for _ in range(self.nvals)] if self.flags & _lib.GB_COUNT else None
         sizes = DeviceColumn.empty(rows, np.int64) if self.flags & _lib.GB_SIZE else None
         return DeviceColumn.empty(rows, np.int64), sums, cnts, sizes

@@ -615,12 +615,22 @@ class DataFrameGroupBy:
     def max(self, numeric_only=False, min_count=-1):
         return self._wrap_aggregation(type(self._query_compiler).groupby_max, numeric_only)
 
+    def first(self, numeric_only=False, min_count=-1, skipna=True):
+        """The first non-NaN value of every column per group (every row's value under ``skipna=False``), passed on as
+        modin/pandas/groupby.py:904-915 does."""
+        return self._wrap_aggregation(type(self._query_compiler).groupby_first, numeric_only,
+                                      agg_kwargs=dict(min_count=min_count, skipna=skipna))  # fmt: skip
+
+    def last(self, numeric_only=False, min_count=-1, skipna=True):
+        return self._wrap_aggregation(type(self._query_compiler).groupby_last, numeric_only,
+                                      agg_kwargs=dict(min_count=min_count, skipna=skipna))  # fmt: skip
+
     def size(self):
         res = self._wrap_aggregation(type(self._query_compiler).groupby_size)
         return Series(query_compiler=res._query_compiler)
 
     def agg(self, func, *args, **kwargs):
-        if isinstance(func, str) and func in ("sum", "count", "mean", "size", "min", "max"):
+        if isinstance(func, str) and func in ("sum", "count", "mean", "size", "min", "max", "first", "last"):
             return getattr(self, func)()
         if isinstance(func, dict):
             return self._dict_agg(func)

@@ -23,7 +23,7 @@ from __future__ import annotations
 import numpy as np
 import pandas
 
-from . import algebra
+from . import algebra, dist
 from . import groupkeys as gk
 from .block import concat_cols
 from .dataframe import B200Dataframe
@@ -52,14 +52,38 @@ def _dtypes_sum(dtypes: pandas.Series, *func_args, **func_kwargs):
     return np.result_type(*dtypes.values) if len(dtypes) else np.dtype("float64")
 
 
+def _position_agg_skipna(agg: str, agg_kwargs) -> bool:
+    """``skipna`` of ``groupby.first`` / ``last`` from the ``agg_kwargs`` Modin passes (modin/pandas/groupby.py:904-915).
+    ``min_count`` of -1, 0 or 1 leaves the result as it is (every group has a row); a larger one makes pandas put NaN
+    into groups with fewer values and change the dtypes of int64 / bool columns, which is not on the device path."""
+    kw = dict(agg_kwargs or {})
+    skipna, min_count = kw.pop("skipna", True), kw.pop("min_count", -1)
+    if kw:
+        raise NotImplementedError(f"groupby.{agg}({', '.join(kw)}=) is not on the B200 path")
+    if not isinstance(skipna, (bool, np.bool_)):
+        raise ValueError(f"skipna must be a boolean, got {skipna!r}")
+    if min_count not in (-1, 0, 1):
+        raise NotImplementedError(f"groupby.{agg}(min_count={min_count!r}) is not on the B200 path")
+    return bool(skipna)
+
+
 def _groupby_reduce(agg: str):
     """``qc.groupby_<agg>`` (qc.py:3741-3748, alg/groupby.py) over device blocks.  ``by`` is a query compiler of key
-    columns with the frame's rows; ``key_names`` replaces the names of the result's keys (``groupby(level=)``)."""
+    columns with the frame's rows; ``key_names`` replaces the names of the result's keys (``groupby(level=)``).
+    ``agg_kwargs`` are read by first / last only (``skipna``, ``min_count``); the other aggregations ignore them."""
     map_f, red_f = DevGroupbyMap(agg), DevGroupbyReduce(agg)
 
     def caller(query_compiler, by, axis, groupby_kwargs, agg_args, agg_kwargs, drop=False, key_names=None, **kwargs):
+        if by is None and groupby_kwargs.get("level") is not None and hasattr(query_compiler, "_b200_level_key"):
+            # groupby(level=) through the plug-in: its query compiler turns the row labels into the key column
+            by, name = query_compiler._b200_level_key(groupby_kwargs["level"])
+            key_names = [name]
         if axis != 0 or not isinstance(by, type(query_compiler)) or len(by.columns) < 1:
             raise NotImplementedError("device groupby: key columns of the same frame, axis=0")
+        fns = (map_f, red_f)
+        if agg in ("first", "last"):
+            skipna = _position_agg_skipna(agg, agg_kwargs)
+            fns = (DevGroupbyMap(agg, skipna=skipna), DevGroupbyReduce(agg, skipna=skipna))
         frame, by_frame = query_compiler._modin_frame, by._modin_frame
         # a float64 key or several int64 keys: the single-key groupby runs on their int64 image and the G result keys
         # are restored afterwards (groupkeys.py); one int64 key is its own image
@@ -74,7 +98,7 @@ def _groupby_reduce(agg: str):
             frame = query_compiler.getitem_column_array(keep)._modin_frame
         # the functors themselves, not lambdas around them: the partition manager recognises them and fuses map +
         # reduce into one direct-addressed table per GPU when the key range allows (pm.groupby_reduce)
-        new_frame = frame.groupby_reduce(axis, by_frame, map_f, red_f)
+        new_frame = frame.groupby_reduce(axis, by_frame, *fns)
         if image is not None or key_names is not None:
             blocks = gk.restore_keys([row[0].get() for row in new_frame._partitions], image,
                                      groupby_kwargs.get("dropna", True), key_names)  # fmt: skip
@@ -184,8 +208,10 @@ def device_operations(alg):
         groupby_mean = _groupby_reduce("mean")
         groupby_min = _groupby_reduce("min")
         groupby_max = _groupby_reduce("max")
+        groupby_first = _groupby_reduce("first")
+        groupby_last = _groupby_reduce("last")
 
-        _DEVICE_AGGS = ("sum", "count", "size", "mean", "min", "max")
+        _DEVICE_AGGS = ("sum", "count", "size", "mean", "min", "max", "first", "last")
 
         def groupby_agg(self, by, agg_func, axis, groupby_kwargs, agg_args, agg_kwargs, how="axis_wise", drop=False,
                         series_groupby=False):  # fmt: skip
@@ -196,7 +222,7 @@ def device_operations(alg):
             ask for it; every result carries the same ascending group keys, so the result blocks are zipped
             column-wise (buffers shared) in the dictionary's order.  A function name alone goes to its registered
             template.  Anything else has no device form and is refused -- there is no pandas block to fall back to."""
-            if how != "axis_wise" or agg_args or agg_kwargs:
+            if how != "axis_wise" or agg_args or (agg_kwargs and agg_func not in ("first", "last")):
                 raise NotImplementedError(f"groupby ({how}) with extra arguments is not on the B200 path")
             if isinstance(agg_func, str) and agg_func in self._DEVICE_AGGS:
                 return getattr(self, f"groupby_{agg_func}")(
@@ -208,6 +234,10 @@ def device_operations(alg):
                 raise NotImplementedError("device groupby: key columns of the same frame, axis=0")
             spec = {col: fn[0] if isinstance(fn, (list, tuple)) and len(fn) == 1 else fn for col, fn in agg_func.items()}
             by_func = gk.split_aggregations(spec, self.columns, set(by.columns) if drop else ())
+            if len(by_func) > 1 and set(by_func) & {"first", "last"} and dist.is_distributed():
+                # across ranks the fused dense path of the other functions and the key-range exchange of first / last
+                # give each rank a different key range
+                raise NotImplementedError("groupby.agg mixing first / last with other functions across ranks")
             if any(isinstance(fn, (list, tuple)) for fn in agg_func.values()):
                 raise NotImplementedError("groupby.agg with lists of functions (two-level result columns)")
             kw = dict(groupby_kwargs, as_index=True)
