@@ -39,8 +39,9 @@ extern "C" {
 
 /* 2: round 2 (key statistics, async dense emit, expand / concat / comm entry points); 3: + the Fold template's
  * cumulative scans (mb200_cum_*); 4: + MB200_GB_FIRST / MB200_GB_LAST group tables (row positions, NULL value
- * columns).  Checked by the binding at load time (modin_b200/_lib.py). */
-#define MB200_ABI_VERSION 4
+ * columns); 5: + MB200_GB_ARGMIN / MB200_GB_ARGMAX group tables and mb200_gb_accumulate_arg.  Checked by the binding
+ * at load time (modin_b200/_lib.py). */
+#define MB200_ABI_VERSION 5
 #define MB200_MAX_COLS 32 /* max columns per launch == Modin's MinColumnPartitionSize (envvars.py:1149-1190) */
 
 typedef void* mb200_stream_t;
@@ -135,7 +136,11 @@ enum mb200_gb_flags {
   /* row positions (int64) instead of values; each excludes SUM / COUNT / MIN / MAX and the other (SIZE may be set):
    * see mb200_gb_accumulate and mb200_gb_emit */
   MB200_GB_FIRST = 32, /* acc[g][v]   = min(position) over the rows whose value in column v is not NaN */
-  MB200_GB_LAST = 64   /* acc[g][v]   = max(position) over the same rows                               */
+  MB200_GB_LAST = 64,  /* acc[g][v]   = max(position) over the same rows                               */
+  /* the first row holding the group's extreme value; each excludes every other flag (see mb200_gb_accumulate_arg):
+   * cnt[g][v] = min / max of the value's order-preserving int64 image, acc[g][v] = min(position) of the rows holding it */
+  MB200_GB_ARGMIN = 128,
+  MB200_GB_ARGMAX = 256
 };
 
 /* ======================= runtime / memory ================================== */
@@ -263,11 +268,19 @@ int mb200_gb_accumulate(mb200_gb_table* table, const int64_t* keys, const void* 
                         int64_t nrows, mb200_stream_t stream);
 /* Merge partial tables (keys + partial sums/counts/sizes as produced by mb200_gb_emit) into
  * `table`: replaces GroupByReduce.reduce alg/groupby.py:211-300 (groupby(level=0).sum()).
- * Refused for FIRST / LAST tables: positions of one table mean nothing in another; their reduce re-accumulates
- * the concatenated partial VALUES as raw rows. */
+ * Refused for FIRST / LAST and ARGMIN / ARGMAX tables: positions of one table mean nothing in another; their reduce
+ * re-accumulates the concatenated partial VALUES as raw rows.  mb200_gb_accumulate refuses ARGMIN / ARGMAX tables. */
 int mb200_gb_merge_partial(mb200_gb_table* table, const int64_t* keys,
                            const void* const* sums, const void* const* cnts,
                            const int64_t* sizes, int64_t npartial, mb200_stream_t stream);
+/* groupby.idxmin / idxmax of an ARGMIN / ARGMAX table: keys[nrows] int64, vals[nvals][nrows] float64 or int64 (bit
+ * v of i64_mask set: column v is int64), row positions 0 .. nrows-1.  Two passes on `stream`: every non-NaN value
+ * takes the min / max of its image into cnt (float64: f64_to_ordered with -0.0 folded into +0.0, so the two zeros
+ * tie; int64: the value itself), then every row whose image equals its group's extreme takes the min of its position
+ * into acc.  The maximum is unique and so is the smallest position holding it, so the result does not depend on the
+ * order of the atomics.  Called once per table: a second call is refused (positions would not run on). */
+int mb200_gb_accumulate_arg(mb200_gb_table* table, const int64_t* keys, const void* const* vals, uint32_t i64_mask,
+                            int64_t nrows, mb200_stream_t stream);
 /* Synchronises `stream`; returns number of groups and whether capacity was exceeded. */
 int mb200_gb_ngroups(mb200_gb_table* table, int64_t* ngroups, int* overflow,
                      mb200_stream_t stream);
@@ -275,8 +288,8 @@ int mb200_gb_ngroups(mb200_gb_table* table, int64_t* ngroups, int* overflow,
 size_t mb200_gb_emit_scratch_bytes(int64_t ngroups);
 /* Write the result block: out_keys[ngroups] (ascending iff sort), out_sums[nvals][ngroups],
  * out_cnts[nvals][ngroups] (int64, may be NULL), out_sizes[ngroups] (may be NULL).
- * FIRST / LAST tables write int64 positions into out_sums, -1 where the group has no non-NaN value in the column
- * (mb200_take turns -1 into NaN). */
+ * FIRST / LAST and ARGMIN / ARGMAX tables write int64 positions into out_sums, -1 where the group has no non-NaN
+ * value in the column (mb200_take turns -1 into NaN). */
 int mb200_gb_emit(mb200_gb_table* table, int64_t ngroups, int sort, int64_t* out_keys,
                   void* const* out_sums, void* const* out_cnts, int64_t* out_sizes,
                   void* scratch, mb200_stream_t stream);

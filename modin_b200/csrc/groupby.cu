@@ -86,12 +86,14 @@ struct mb200_gb_table {
   void* arena;
   size_t arena_bytes;
   long long rows;  // rows accumulated so far: the position of the next accumulate call's first row (FIRST / LAST)
+  int arg_filled;  // ARGMIN / ARGMAX: mb200_gb_accumulate_arg has run (it runs once per table)
 };
 
 namespace mb200 {
 
 constexpr int kGbThreads = 256;
 constexpr int kGbWarps = kGbThreads / 32;
+constexpr int kGbArg = MB200_GB_ARGMIN | MB200_GB_ARGMAX;  // groupby.idxmin / idxmax tables
 constexpr int kColStride = 34;  // doubles; 34 = 2 (mod 16) -> conflict-free transposed reads
 // TMA-staged kernel
 constexpr int kTileRows = 256;
@@ -831,9 +833,10 @@ __global__ void gb_emit_kernel(const __grid_constant__ EmitParams p) {
   for (int v = 0; v < p.nvals; ++v) {
     if (p.out_sums[v] && p.acc) {
       double val = p.acc[(size_t)g * p.vstride + v];
-      if (p.flags & (MB200_GB_FIRST | MB200_GB_LAST)) {  // int64 position; -1: no non-NaN value in the group
+      if (p.flags & (MB200_GB_FIRST | MB200_GB_LAST | MB200_GB_ARGMIN | MB200_GB_ARGMAX)) {
+        // int64 position; -1: no non-NaN value in the group (every position table but LAST's starts at INT64_MAX)
         const long long o = __double_as_longlong(val);
-        const bool empty = (p.flags & MB200_GB_FIRST) ? (o == 0x7fffffffffffffffLL) : (o == (long long)0x8000000000000000ULL);
+        const bool empty = (p.flags & MB200_GB_LAST) ? (o == (long long)0x8000000000000000ULL) : (o == 0x7fffffffffffffffLL);
         val = __longlong_as_double(empty ? -1LL : o);
       } else if (p.flags & (MB200_GB_MIN | MB200_GB_MAX)) {
         const long long o = __double_as_longlong(val);
@@ -1203,6 +1206,280 @@ static int gb_launch(mb200_gb_table* t, const long long* keys, const void* const
   return launch_ldg<0, false>(p, dp, st);
 }
 
+
+// ---------------------------------------------------------------- ARGMIN / ARGMAX tables (groupby.idxmin / idxmax)
+// Two passes over the same raw rows, on one stream.  Pass 1 takes, per (group, column), the min / max of the values'
+// order-preserving int64 images into `cnt` (RED.MIN / MAX.S64, as min / max do); pass 2 takes the min of the positions
+// of the rows whose image equals that final extreme into `acc`.  The extreme is unique and so is the smallest
+// position holding it: the result is exact whatever the order of the atomics.  A float64 image folds -0.0 into +0.0
+// (the two zeros tie, as in pandas); an int64 image is the value itself, so a group whose values all equal the
+// "no value yet" sentinel (INT64_MIN for ARGMAX) still has rows equal to its extreme and resolves in pass 2.
+// New kernels: the gb_accumulate* instantiations are untouched.
+__device__ __forceinline__ bool arg_image(double x, bool i64, long long& img) {
+  if (i64) {
+    img = __double_as_longlong(x);
+    return true;
+  }
+  if (x != x) return false;  // NaN: skipped
+  img = (x == 0.0) ? 0LL : f64_to_ordered(x);
+  return true;
+}
+__device__ __forceinline__ long long ld_relaxed_s64(const long long* p) {
+  long long v;
+  asm volatile("ld.relaxed.gpu.global.s64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+
+// direct loads, dense or hashed tables: the mapping of gb_accumulate_kernel (warp = 32 rows, value tile transposed
+// through shared memory, 8 lanes per row = 8 columns of one group's 64-byte row of the table)
+// (pass 1 at 4 CTAs per SM: at 5 the 48-register budget spills around the insert path, as the accumulate kernel does)
+template <int PASS>
+__global__ void __launch_bounds__(kGbThreads, PASS == 1 ? 4 : 5) gb_arg_kernel(const __grid_constant__ GbParams p,
+                                                                 const unsigned int i64_mask) {
+  __shared__ double s_tile[kGbWarps][8 * kColStride];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long nchunks = (p.nrows + 31) >> 5;
+  const long long wstride = (long long)gridDim.x * kGbWarps;
+  const int gcap = (int)p.gcap;
+  const uint64_t pol = l2_policy_evict_first();
+  const bool amax = p.flags & MB200_GB_ARGMAX;
+  long long* const img_tab = p.cnt;
+  long long* const pos_tab = reinterpret_cast<long long*>(p.acc);
+  for (long long ch = (long long)blockIdx.x * kGbWarps + warp; ch < nchunks; ch += wstride) {
+    const long long base = ch << 5;
+    const long long row = base + lane;
+    const bool valid = row < p.nrows;
+    long long k = valid ? ldg_stream_i64(p.keys + row, pol) : 0;
+    double x[8];
+    {
+      const int nc = p.nvals < 8 ? p.nvals : 8;
+#pragma unroll
+      for (int c = 0; c < 8; ++c)
+        x[c] = (c < nc && valid) ? ldg_stream_f64(static_cast<const double*>(p.vals[c]) + row, pol) : 0.0;
+    }
+    {
+      const long long k0 = __shfl_sync(0xffffffffu, k, 0);  // rows past the end join lane 0's peer group
+      k = valid ? k : k0;
+    }
+    const int gid = resolve_gid(p, k, 0);  // pass 2: every key is in the table already, nothing is inserted
+    if (PASS == 1 && p.dense && p.nvals == 0 && valid && gid < gcap) dense_mark(p, gid);
+    for (int c0 = 0; c0 < p.nvals; c0 += 8) {
+      const int nc = (p.nvals - c0) < 8 ? (p.nvals - c0) : 8;
+      if (c0 > 0) {
+#pragma unroll
+        for (int c = 0; c < 8; ++c)
+          x[c] = (c < nc && valid) ? ldg_stream_f64(static_cast<const double*>(p.vals[c0 + c]) + row, pol) : 0.0;
+      }
+      double* tile = s_tile[warp];
+#pragma unroll
+      for (int c = 0; c < 8; ++c) tile[c * kColStride + lane] = x[c];
+      __syncwarp();
+      const int c = lane & 7;
+      const bool is_i64 = c < nc && ((i64_mask >> (c0 + c)) & 1u);
+      unsigned int seen = 0, rowok = 0;
+      int gs[8];
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        const int r = 4 * kk + (lane >> 3);
+        const int g = __shfl_sync(0xffffffffu, gid, r);
+        const double xv = tile[c * kColStride + r];
+        const bool rok = (base + r < p.nrows) && g < gcap;
+        gs[kk] = g;
+        if (rok) rowok |= 1u << kk;
+        long long img;
+        if (rok && c < nc && arg_image(xv, is_i64, img)) {
+          const size_t o = (size_t)g * p.vstride + c0 + c;
+          if (PASS == 1) {
+            seen |= 1u << kk;
+            if (amax) red_max_s64(img_tab + o, img);
+            else red_min_s64(img_tab + o, img);
+          } else if (img == __ldg(img_tab + o)) {
+            // positions only fall: a row at or past the current minimum cannot win, and skipping it keeps a run of
+            // equal extremes (bool columns, few distinct int64 values) from serialising on one address
+            const long long pos = base + r;
+            if (pos < ld_relaxed_s64(pos_tab + o)) red_min_s64(pos_tab + o, pos);
+          }
+        }
+      }
+      if (PASS == 1 && p.dense) {  // rows without a value in these columns mark their presence byte
+        seen |= __shfl_xor_sync(0xffffffffu, seen, 1);
+        seen |= __shfl_xor_sync(0xffffffffu, seen, 2);
+        seen |= __shfl_xor_sync(0xffffffffu, seen, 4);
+        const unsigned int unseen = ~seen & rowok;
+        if (c == 0 && unseen) {
+#pragma unroll
+          for (int kk = 0; kk < 8; ++kk)
+            if ((unseen >> kk) & 1u) dense_mark(p, gs[kk]);
+        }
+      }
+      __syncwarp();
+    }
+  }
+}
+
+// low-cardinality dense tables (the ranges gb_accumulate_smem_kernel serves): per-CTA shared-memory tables.
+// Pass 1: shared atomics on the images in `nrep` replicas (lane l of a warp works on replica l & (nrep - 1)), folded
+// into the global images once per CTA; every row marks its key present.  Pass 2: each CTA loads the final images of
+// the range into shared memory and takes the position minimum in the replicas, folded into the global positions once.
+// Layout: acc_off = replicas (images in pass 1, positions in pass 2), cnt_off = the final images (pass 2), present_off.
+template <int PASS>
+__global__ void __launch_bounds__(kSmemThreads, 1) gb_arg_smem_kernel(const __grid_constant__ GbParams p,
+                                                                        const SmemTableLayout lay,
+                                                                        const unsigned int i64_mask) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  long long* s_rep = reinterpret_cast<long long*>(smem_raw + lay.acc_off);
+  long long* s_img = reinterpret_cast<long long*>(smem_raw + lay.cnt_off);
+  unsigned char* s_present = smem_raw + lay.present_off;
+  const int tid = threadIdx.x;
+  const int nv = p.nvals, vs = p.vstride, svs = lay.svs;
+  const int R = (int)p.gcap;
+  const int nrep = lay.nrep, rstride = lay.rstride;
+  const bool amax = p.flags & MB200_GB_ARGMAX;
+  const long long init = (PASS == 1 && amax) ? (long long)0x8000000000000000ULL : 0x7fffffffffffffffLL;
+  for (int i = tid; i < nrep * rstride; i += kSmemThreads) s_rep[i] = init;
+  if (PASS == 1) {
+    for (int i = tid; i < R; i += kSmemThreads) s_present[i] = 0;
+  } else {
+    for (int i = tid; i < R * vs; i += kSmemThreads) {
+      const int g = i / vs, cc = i - g * vs;
+      if (cc < nv) s_img[g * svs + cc] = p.cnt[i];
+    }
+  }
+  __syncthreads();
+  const uint64_t pol = l2_policy_evict_first();
+  const int rbase = (tid & (nrep - 1)) * rstride;
+  const long long stride = (long long)gridDim.x * kSmemThreads;
+  for (long long row = (long long)blockIdx.x * kSmemThreads + tid; row < p.nrows; row += stride) {
+    const long long key = ldg_stream_i64(p.keys + row, pol);
+    double x[8];
+    {
+      const int nc = nv < 8 ? nv : 8;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) x[c] = (c < nc) ? ldg_stream_f64(static_cast<const double*>(p.vals[c]) + row, pol) : 0.0;
+    }
+    const unsigned long long d = (unsigned long long)key - (unsigned long long)p.kbase;
+    if (d >= (unsigned long long)R) {
+      p.meta->overflow = 1;  // key outside the declared range
+      continue;
+    }
+    const int gid = (int)d;
+    if (PASS == 1 && !s_present[gid]) s_present[gid] = 1;
+    for (int c0 = 0; c0 < nv; c0 += 8) {
+      const int nc = (nv - c0) < 8 ? (nv - c0) : 8;
+      if (c0 > 0) {
+#pragma unroll
+        for (int c = 0; c < 8; ++c)
+          x[c] = (c < nc) ? ldg_stream_f64(static_cast<const double*>(p.vals[c0 + c]) + row, pol) : 0.0;
+      }
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        long long img;
+        if (c < nc && arg_image(x[c], (i64_mask >> (c0 + c)) & 1u, img)) {
+          const int o = gid * svs + c0 + c;
+          if (PASS == 1) {
+            if (amax) atomicMax(&s_rep[rbase + o], img);
+            else atomicMin(&s_rep[rbase + o], img);
+          } else if (img == s_img[o] && row < s_rep[rbase + o]) {
+            atomicMin(&s_rep[rbase + o], row);
+          }
+        }
+      }
+    }
+  }
+  __syncthreads();
+  for (int i = tid; i < R * vs; i += kSmemThreads) {
+    const int g = i / vs, cc = i - g * vs;
+    if (cc >= nv || (PASS == 1 && !s_present[g])) continue;
+    const int o = g * svs + cc;
+    long long a = s_rep[o];
+    for (int r = 1; r < nrep; ++r) {
+      const long long b = s_rep[r * rstride + o];
+      a = (PASS == 1 && amax) ? (b > a ? b : a) : (b < a ? b : a);
+    }
+    if (a == init) continue;
+    if (PASS == 2) red_min_s64(reinterpret_cast<long long*>(p.acc) + i, a);
+    else if (amax) red_max_s64(p.cnt + i, a);
+    else red_min_s64(p.cnt + i, a);
+  }
+  if (PASS == 1)
+    for (int g = tid; g < R; g += kSmemThreads)
+      if (s_present[g]) reinterpret_cast<unsigned char*>(p.present)[g] = 1;
+}
+
+template <int PASS>
+static int launch_arg_ldg(const GbParams& p, unsigned int i64_mask, const DevProps& dp, cudaStream_t st) {
+  int occ = 0;
+  MB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, gb_arg_kernel<PASS>, kGbThreads, 0));
+  const long long nchunks = (p.nrows + 31) / 32;
+  long long grid = (long long)dp.sm_count * (occ < 1 ? 1 : occ);
+  const long long need = (nchunks + kGbWarps - 1) / kGbWarps;
+  if (grid > need) grid = need;
+  gb_arg_kernel<PASS><<<(unsigned)grid, kGbThreads, 0, st>>>(p, i64_mask);
+  MB_LAUNCH_CHECK("gb_arg_kernel");
+  return 0;
+}
+
+static int gb_arg_launch(mb200_gb_table* t, const long long* keys, const void* const* vals, unsigned int i64_mask,
+                         long long nrows, cudaStream_t st) {
+  if (nrows == 0) return 0;
+  DevProps dp;
+  if (int rc = dev_props(&dp)) return rc;
+  GbParams p;
+  memset(&p, 0, sizeof(p));
+  p.slots = t->slots;
+  p.mask = (unsigned int)(t->cap - 1);
+  p.cap = t->cap;
+  p.acc = t->acc;
+  p.cnt = t->cnt;
+  p.gcap = t->gcap;
+  p.nvals = t->nvals;
+  p.vstride = t->vstride;
+  p.flags = t->flags;
+  p.meta = t->meta;
+  p.dense = t->dense;
+  p.kbase = t->kbase;
+  p.present = t->present;
+  p.keys = keys;
+  p.nrows = nrows;
+  for (int c = 0; c < t->nvals; ++c) {
+    p.vals[c] = vals[c];
+    if (!p.vals[c]) return fail("mb200_gb_accumulate_arg", "null value column");
+  }
+  if (t->dense && !(getenv("MB200_GB_SMEM") && getenv("MB200_GB_SMEM")[0] == '0')) {
+    SmemTableLayout lay;
+    memset(&lay, 0, sizeof(lay));
+    lay.svs = t->vstride + 1;
+    const size_t elems1 = (size_t)t->gcap * lay.svs;
+    lay.rstride = (int)(((elems1 + 15) & ~(size_t)15) + 1);
+    size_t off = 0;
+    for (int nrep = 32; nrep >= 1; nrep >>= 1) {
+      lay.nrep = nrep;
+      lay.acc_off = 0;
+      off = (((size_t)nrep * lay.rstride * 8) + 15) & ~(size_t)15;
+      lay.cnt_off = (unsigned)off;
+      off += elems1 * 8;
+      lay.present_off = (unsigned)off;
+      off += ((size_t)t->gcap + 15) & ~(size_t)15;
+      lay.total = (unsigned)off;
+      if (off <= dp.smem_optin) break;
+    }
+    if (off <= dp.smem_optin) {
+      long long grid = dp.sm_count;
+      const long long need = (nrows + kSmemThreads - 1) / kSmemThreads;
+      if (grid > need) grid = need;
+      MB_CUDA(cudaFuncSetAttribute(gb_arg_smem_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)off));
+      MB_CUDA(cudaFuncSetAttribute(gb_arg_smem_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)off));
+      gb_arg_smem_kernel<1><<<(unsigned)grid, kSmemThreads, off, st>>>(p, lay, i64_mask);
+      MB_LAUNCH_CHECK("gb_arg_smem_kernel");
+      gb_arg_smem_kernel<2><<<(unsigned)grid, kSmemThreads, off, st>>>(p, lay, i64_mask);
+      MB_LAUNCH_CHECK("gb_arg_smem_kernel");
+      return 0;
+    }
+  }
+  if (int rc = launch_arg_ldg<1>(p, i64_mask, dp, st)) return rc;
+  return launch_arg_ldg<2>(p, i64_mask, dp, st);
+}
+
 }  // namespace mb200
 
 using namespace mb200;
@@ -1229,8 +1506,8 @@ extern "C" int mb200_gb_create_dense(mb200_gb_table** table, int64_t key_min, in
   if (range == 0 || range > (1ULL << 29)) return fail("mb200_gb_create_dense", "key range above 2^29");
   DenseArrays ext{acc, cnt, size, present};
   if (present) {
-    const bool need_acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST);
-    if ((need_acc && !acc) || ((flags & MB200_GB_COUNT) && !cnt) || ((flags & MB200_GB_SIZE) && !size))
+    const bool need_acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST | kGbArg);
+    if ((need_acc && !acc) || ((flags & (MB200_GB_COUNT | kGbArg)) && !cnt) || ((flags & MB200_GB_SIZE) && !size))
       return fail("mb200_gb_create_dense", "caller-owned arrays: every array the flags need must be given");
     if (!aligned16(acc) || !aligned16(cnt) || !aligned16(size) || !aligned16(present))
       return fail("mb200_gb_create_dense", "caller-owned arrays must be 16-byte aligned");
@@ -1252,8 +1529,8 @@ extern "C" int mb200_gb_adopt_dense(mb200_gb_table** table, int64_t key_min, int
   if (key_max < key_min) return fail("mb200_gb_adopt_dense", "empty key range");
   const unsigned long long range = (unsigned long long)key_max - (unsigned long long)key_min + 1ULL;
   if (range == 0 || range > (1ULL << 29)) return fail("mb200_gb_adopt_dense", "key range above 2^29");
-  const bool need_acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST);
-  if (!present || (need_acc && !acc) || ((flags & MB200_GB_COUNT) && !cnt) || ((flags & MB200_GB_SIZE) && !size))
+  const bool need_acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST | kGbArg);
+  if (!present || (need_acc && !acc) || ((flags & (MB200_GB_COUNT | kGbArg)) && !cnt) || ((flags & MB200_GB_SIZE) && !size))
     return fail("mb200_gb_adopt_dense", "every array the flags need must be given");
   if (!aligned16(acc) || !aligned16(cnt) || !aligned16(size) || !aligned16(present))
     return fail("mb200_gb_adopt_dense", "arrays must be 16-byte aligned");
@@ -1312,6 +1589,8 @@ static int gb_create_impl(mb200_gb_table** table, int64_t group_capacity, int nv
       (flags & (MB200_GB_SUM | MB200_GB_COUNT | MB200_GB_MIN | MB200_GB_MAX) ||
        (flags & (MB200_GB_FIRST | MB200_GB_LAST)) == (MB200_GB_FIRST | MB200_GB_LAST)))
     return fail("mb200_gb_create", "FIRST / LAST exclude every other accumulator flag");
+  if ((flags & kGbArg) && flags != MB200_GB_ARGMIN && flags != MB200_GB_ARGMAX)
+    return fail("mb200_gb_create", "ARGMIN / ARGMAX exclude every other flag");
   DevProps dp;
   if (int rc = dev_props(&dp)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
@@ -1349,9 +1628,9 @@ static int gb_create_impl(mb200_gb_table** table, int64_t group_capacity, int nv
   } else {
     const size_t slot_b = ((size_t)t->cap * sizeof(Slot) + 255) & ~(size_t)255;
     const size_t acc_b = (accb + 255) & ~(size_t)255;
-    const bool has_acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST);
+    const bool has_acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST | kGbArg);
     const size_t size_b = (((size_t)t->gcap * 8) + 255) & ~(size_t)255;
-    t->arena_bytes = slot_b + (has_acc ? acc_b : 0) + ((flags & MB200_GB_COUNT) ? acc_b : 0) +
+    t->arena_bytes = slot_b + (has_acc ? acc_b : 0) + ((flags & (MB200_GB_COUNT | kGbArg)) ? acc_b : 0) +
                      ((flags & MB200_GB_SIZE) ? size_b : 0);
     MB_TRY(cudaMallocAsync(&t->arena, t->arena_bytes, st));
     char* a = static_cast<char*>(t->arena);
@@ -1361,7 +1640,7 @@ static int gb_create_impl(mb200_gb_table** table, int64_t group_capacity, int nv
       t->acc = reinterpret_cast<double*>(a);
       a += acc_b;
     }
-    if (flags & MB200_GB_COUNT) {
+    if (flags & (MB200_GB_COUNT | kGbArg)) {  // ARGMIN / ARGMAX: the extreme images
       t->cnt = reinterpret_cast<long long*>(a);
       a += acc_b;
     }
@@ -1380,14 +1659,21 @@ static int gb_create_impl(mb200_gb_table** table, int64_t group_capacity, int nv
     } else {
       MB_TRY(cudaMemsetAsync(t->acc, 0, accb, st));
     }
-  } else if (flags & (MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST)) {
+  } else if (flags & (MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST | kGbArg)) {
     if (!t->borrowed && dense) MB_TRY(cudaMallocAsync((void**)&t->acc, accb, st));
     // "no value yet": INT64_MAX = bytes ff..ff 7f for min is not a byte pattern; use the fill kernel
     gb_fill_kernel<<<(unsigned)dp.sm_count * 4, 256, 0, st>>>(reinterpret_cast<long long*>(t->acc),
                                                              (long long)(accb / 8),
-                                                             (flags & (MB200_GB_MIN | MB200_GB_FIRST))
+                                                             (flags & (MB200_GB_MIN | MB200_GB_FIRST | kGbArg))
                                                                  ? 0x7fffffffffffffffLL
                                                                  : (long long)0x8000000000000000ULL);
+    MB_TRY(cudaGetLastError());
+    g_launches.fetch_add(1);
+  }
+  if ((flags & kGbArg) && init_arrays) {  // extreme images start below / above every image
+    if (!t->borrowed && dense) MB_TRY(cudaMallocAsync((void**)&t->cnt, accb, st));
+    gb_fill_kernel<<<(unsigned)dp.sm_count * 4, 256, 0, st>>>(
+        t->cnt, (long long)(accb / 8), (flags & MB200_GB_ARGMAX) ? (long long)0x8000000000000000ULL : 0x7fffffffffffffffLL);
     MB_TRY(cudaGetLastError());
     g_launches.fetch_add(1);
   }
@@ -1442,6 +1728,7 @@ extern "C" int mb200_gb_accumulate(mb200_gb_table* t, const int64_t* keys, const
   if (!t) return fail("mb200_gb_accumulate", "null table");
   if (nrows < 0) return fail("mb200_gb_accumulate", "negative nrows");
   if (nrows > 0 && !keys) return fail("mb200_gb_accumulate", "null keys");
+  if (t->flags & kGbArg) return fail("mb200_gb_accumulate", "ARGMIN / ARGMAX tables take mb200_gb_accumulate_arg");
   if (int rc = gb_launch(t, reinterpret_cast<const long long*>(keys), vals, nullptr, nullptr, nrows, false,
                          (cudaStream_t)stream))
     return rc;
@@ -1455,18 +1742,36 @@ extern "C" int mb200_gb_merge_partial(mb200_gb_table* t, const int64_t* keys, co
   if (!t) return fail("mb200_gb_merge_partial", "null table");
   if (npartial < 0) return fail("mb200_gb_merge_partial", "negative npartial");
   if (npartial > 0 && !keys) return fail("mb200_gb_merge_partial", "null keys");
+  if (t->flags & kGbArg) return fail("mb200_gb_merge_partial", "ARGMIN / ARGMAX tables do not merge partial tables");
   return gb_launch(t, reinterpret_cast<const long long*>(keys), sums, cnts, reinterpret_cast<const long long*>(sizes),
                    npartial, true, (cudaStream_t)stream);
+}
+
+extern "C" int mb200_gb_accumulate_arg(mb200_gb_table* t, const int64_t* keys, const void* const* vals,
+                                       uint32_t i64_mask, int64_t nrows, mb200_stream_t stream) {
+  if (!t) return fail("mb200_gb_accumulate_arg", "null table");
+  if (!(t->flags & kGbArg)) return fail("mb200_gb_accumulate_arg", "not an ARGMIN / ARGMAX table");
+  if (t->arg_filled) return fail("mb200_gb_accumulate_arg", "an ARGMIN / ARGMAX table is filled by one call");
+  if (nrows < 0) return fail("mb200_gb_accumulate_arg", "negative nrows");
+  if (nrows > 0 && !keys) return fail("mb200_gb_accumulate_arg", "null keys");
+  if (nrows > 0 && t->nvals > 0 && !vals) return fail("mb200_gb_accumulate_arg", "null value columns");
+  if (int rc = gb_arg_launch(t, reinterpret_cast<const long long*>(keys), vals, i64_mask, nrows, (cudaStream_t)stream))
+    return rc;
+  t->arg_filled = 1;
+  t->rows = nrows;
+  return 0;
 }
 
 static int dense_finalize_presence(mb200_gb_table* t, cudaStream_t st) {
   const long long n = t->win_hi - t->win_lo;
   if (n <= 0) return 0;
   const long long init = (t->flags & MB200_GB_SUM)   ? (long long)0x8000000000000000ULL
-                         : (t->flags & (MB200_GB_MIN | MB200_GB_FIRST)) ? 0x7fffffffffffffffLL
+                         : (t->flags & (MB200_GB_MIN | MB200_GB_FIRST | kGbArg)) ? 0x7fffffffffffffffLL
                                                      : (long long)0x8000000000000000ULL;
+  // ARGMIN / ARGMAX: cnt holds images, not counts; presence is a moved position or a marked byte
   dense_presence_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
-      reinterpret_cast<unsigned char*>(t->present), reinterpret_cast<const long long*>(t->acc), t->cnt, t->size,
+      reinterpret_cast<unsigned char*>(t->present), reinterpret_cast<const long long*>(t->acc),
+      (t->flags & kGbArg) ? nullptr : t->cnt, t->size,
       t->win_lo, t->win_hi, t->nvals, t->vstride, init);
   MB_LAUNCH_CHECK("dense_presence_kernel");
   return 0;

@@ -979,6 +979,40 @@ class DevVar(DevFn):
 _LABEL_EMPTY, _LABEL_I64, _LABEL_F64, _LABEL_REFUSED = 0, 1, 2, 3
 
 
+def _label_kind(block):
+    """(kind code, refusal message) of the block's row labels (``idxmax`` / ``idxmin``, frame-wide and per group)."""
+    if block.nrows == 0:
+        return _LABEL_EMPTY, None
+    if block.has_range_index():
+        return _LABEL_I64, None
+    if block.index_cols:
+        if len(block.index_cols) != 1:
+            return _LABEL_REFUSED, "idxmax / idxmin over several index levels is not on the B200 path"
+        return (_LABEL_F64 if block.index_cols[0].dtype == np.float64 else _LABEL_I64), None
+    idx = block.index_host
+    if isinstance(idx, pandas.MultiIndex):
+        return _LABEL_REFUSED, "idxmax / idxmin over several index levels is not on the B200 path"
+    if idx.dtype.kind not in "if":
+        return _LABEL_REFUSED, f"idxmax / idxmin over {idx.dtype} row labels is not on the B200 path"
+    return (_LABEL_F64 if idx.dtype.kind == "f" else _LABEL_I64), None
+
+
+def _labels(block, kind, pos):
+    """Row labels at the positions ``pos`` (int64 device tensor; -1 gives an arbitrary label)."""
+    t = ops.torch_mod()
+    if kind == _LABEL_EMPTY:
+        return t.zeros_like(pos)
+    p = DeviceColumn(pos, np.int64)
+    if block.has_range_index():
+        return ops.map_columns("add_s", [p], s0=[block.range_start])[0].data
+    if block.index_cols:
+        return ops.take_columns([block.index_cols[0]], p)[0].data
+    host = block.index_host.to_numpy().astype(np.float64 if kind == _LABEL_F64 else np.int64)
+    at = pos.tolist()
+    return t.tensor([host[i] if i >= 0 else 0 for i in at], dtype=t.float64 if kind == _LABEL_F64 else t.int64,
+                    device=pos.device)  # fmt: skip
+
+
 class DevArgReduce(DevFn):
     """``pandas.DataFrame.idxmax / idxmin`` of one FULL column partition -> 1 x W block of row labels: the device body
     of the Reduce template (alg/reduce.py:32-71; qc.py:1101-1102 registers ``Reduce.register(pandas.DataFrame.idxmax
@@ -998,40 +1032,6 @@ class DevArgReduce(DevFn):
             raise ValueError(op)
         self.op = op
 
-    @staticmethod
-    def _label_kind(block):
-        """(kind code, refusal message) of the block's row labels."""
-        if block.nrows == 0:
-            return _LABEL_EMPTY, None
-        if block.has_range_index():
-            return _LABEL_I64, None
-        if block.index_cols:
-            if len(block.index_cols) != 1:
-                return _LABEL_REFUSED, "idxmax / idxmin over several index levels is not on the B200 path"
-            return (_LABEL_F64 if block.index_cols[0].dtype == np.float64 else _LABEL_I64), None
-        idx = block.index_host
-        if isinstance(idx, pandas.MultiIndex):
-            return _LABEL_REFUSED, "idxmax / idxmin over several index levels is not on the B200 path"
-        if idx.dtype.kind not in "if":
-            return _LABEL_REFUSED, f"idxmax / idxmin over {idx.dtype} row labels is not on the B200 path"
-        return (_LABEL_F64 if idx.dtype.kind == "f" else _LABEL_I64), None
-
-    @staticmethod
-    def _labels(block, kind, pos):
-        """Row labels at the W positions ``pos`` (int64 device tensor; -1 gives an arbitrary label)."""
-        t = ops.torch_mod()
-        if kind == _LABEL_EMPTY:
-            return t.zeros_like(pos)
-        p = DeviceColumn(pos, np.int64)
-        if block.has_range_index():
-            return ops.map_columns("add_s", [p], s0=[block.range_start])[0].data
-        if block.index_cols:
-            return ops.take_columns([block.index_cols[0]], p)[0].data
-        host = block.index_host.to_numpy().astype(np.float64 if kind == _LABEL_F64 else np.int64)
-        at = pos.tolist()
-        return t.tensor([host[i] if i >= 0 else 0 for i in at], dtype=t.float64 if kind == _LABEL_F64 else t.int64,
-                        device=pos.device)  # fmt: skip
-
     def _raise_for(self, counts, nrows, skipna):
         """pandas' errors (nanops._maybe_arg_null_out and the empty check), from the counts of the whole axis."""
         if nrows == 0:
@@ -1048,7 +1048,7 @@ class DevArgReduce(DevFn):
         if not block.cols:
             return _reduced_block([], block.columns)
         spans = _spans_ranks(block)
-        kind, refusal = self._label_kind(block)
+        kind, refusal = _label_kind(block)
         if refusal and not spans:
             raise NotImplementedError(refusal)
         t = ops.torch_mod()
@@ -1057,7 +1057,7 @@ class DevArgReduce(DevFn):
         vals, poss, cnts = ops.arg_reduce_columns(self.op, cols, ReduceVariant.get())
         pos = t.cat([p.reshape(1) for p in poss])
         cnt = t.cat([c.reshape(1) for c in cnts])
-        labels = self._labels(block, kind, pos) if not refusal else t.zeros_like(pos)
+        labels = _labels(block, kind, pos) if not refusal else t.zeros_like(pos)
         nrows = block.nrows
         if spans:
             labels, cnt, nrows, kind = self._combine_ranks(vals, labels, cnt, nrows, kind, cols)
@@ -1280,8 +1280,13 @@ _PARTIALS = {
     # row positions, so partials are never merged as tables (no ``merge_partial``)
     "first": _Partial(_lib.GB_FIRST, ("sums",)),
     "last": _Partial(_lib.GB_LAST, ("sums",)),
+    # the partial of idxmax / idxmin holds each group's winning VALUES (bool widened to int64), then the row labels
+    # they came from (``_arg_partial``); the table behind it holds row positions, so partials are never merged as tables
+    "idxmax": _Partial(_lib.GB_ARGMAX, ("sums", "labels")),
+    "idxmin": _Partial(_lib.GB_ARGMIN, ("sums", "labels")),
 }
 _POSITION_AGGS = ("first", "last")
+_ARG_AGGS = ("idxmax", "idxmin")
 
 
 def _partial_cols(agg, sums, cnts, sizes):
@@ -1296,7 +1301,7 @@ def _partial_labels(agg, labels):
         return pandas.Index(["size"])
     if len(arrays) == 1:
         return labels
-    tags = {"sums": "sum", "cnts": "count"}
+    tags = {"sums": "sum", "cnts": "count", "labels": "label"}
     return pandas.MultiIndex.from_tuples([(tags[name], c) for name in arrays for c in labels])
 
 
@@ -1390,20 +1395,72 @@ def _first_last(agg, key: DeviceColumn, vals, skipna: bool, capacity_hint: int):
     return keys, [ops.take_columns([v], pos[s])[0] for v, s in zip(vals, slot_of)]
 
 
+def _arg_positions(agg, key: DeviceColumn, vals, capacity_hint: int):
+    """``groupby.idxmax`` / ``idxmin`` positions: the ascending group keys and, per value column (float64 / int64),
+    the position of the first row holding the group's extreme, -1 where the group has no non-NaN value.  One ARGMAX /
+    ARGMIN table, filled in two exact passes (``mb200_gb_accumulate_arg``)."""
+    flags = _lib.GB_ARGMAX if agg == "idxmax" else _lib.GB_ARGMIN
+    keys, pos, _, _ = ops.hash_aggregate([(key, list(vals))], flags, capacity_hint)
+    return keys, (pos or [])
+
+
+def arg_label_dtype(blocks) -> np.dtype:
+    """The dtype of the labels ``groupby.idxmax`` / ``idxmin`` return for a frame of row blocks: float64 for float
+    row labels, else int64 (also when there are no rows).  Under ``torch.distributed`` the ranks agree on it first --
+    one host integer per rank -- so that a rank without rows gives the same dtype as the others, and every rank
+    refuses string / MultiIndex labels or labels of two kinds together."""
+    from . import dist
+
+    kinds, refusal = set(), None
+    for b in blocks:
+        kind, why = _label_kind(b)
+        kinds.add(kind)
+        refusal = refusal or why
+    code = (1 << 40) * (refusal is not None) + (1 << 20) * (_LABEL_F64 in kinds) + (_LABEL_I64 in kinds)
+    code = dist.control_sum(code) if dist.is_distributed() else code
+    if code >> 40:
+        raise NotImplementedError(refusal or "idxmax / idxmin over string or several levels of row labels is not on "
+                                  "the B200 path")  # fmt: skip
+    if (code >> 20) & 0xFFFFF and code & 0xFFFFF:
+        raise NotImplementedError("idxmax / idxmin on the B200 path need row labels of one kind (int64 or float64)")
+    return np.dtype(np.float64 if (code >> 20) & 0xFFFFF else np.int64)
+
+
+def _arg_partial(agg, key: DeviceColumn, vals, block, label_dtype, capacity_hint: int):
+    """The partial of ``groupby.idxmax`` / ``idxmin`` over one row block: the group keys, then per value column the
+    winning value (NaN when the group has none in this block), then the row label it came from."""
+    vals = ops.cast_columns_i64(vals)
+    keys, pos = _arg_positions(agg, key, vals, capacity_hint)
+    kind, refusal = _label_kind(block)
+    if refusal:
+        raise NotImplementedError(refusal)
+    values = [ops.take_columns([v], p)[0] for v, p in zip(vals, pos)]
+    if kind == _LABEL_EMPTY:
+        labels = [DeviceColumn.empty(len(keys), label_dtype) for _ in pos]
+    else:
+        labels = [DeviceColumn(_labels(block, kind, p.data), label_dtype) for p in pos]
+    return keys, values + labels
+
+
 class DevGroupbyMap(DevFn):
     """GroupByReduce.map (alg/groupby.py:124-208): hash-aggregate one row block against its
-    slice of `by` into a partial table (index = keys, ascending).  ``skipna``: first / last only."""
+    slice of `by` into a partial table (index = keys, ascending).  ``skipna``: first / last only;
+    ``label_dtype``: idxmax / idxmin only (``arg_label_dtype``)."""
 
-    def __init__(self, agg: str, capacity_hint: int = 1 << 20, skipna: bool = True):
+    def __init__(self, agg: str, capacity_hint: int = 1 << 20, skipna: bool = True, label_dtype=np.int64):
         if agg not in _PARTIALS:
             raise NotImplementedError(f"groupby.{agg} is not on the B200 path")
         self.agg = agg
         self.op = f"groupby_{agg}_map"
         self.capacity_hint = capacity_hint
         self.skipna = skipna
+        self.label_dtype = np.dtype(label_dtype)
 
     def __call__(self, block, by_block=None, *args, **kwargs):
         key, key_label, vals, labels = _split_key_values(block, by_block, self.op)
+        if self.agg in _ARG_AGGS:
+            keys, cols = _arg_partial(self.agg, key, vals, block, self.label_dtype, self.capacity_hint)
+            return _group_block(cols, _partial_labels(self.agg, labels), keys, key_label)
         if self.agg in _POSITION_AGGS:
             # the partial is what pandas' groupby.first / last gives for this row block
             keys, cols = _first_last(self.agg, key, vals, self.skipna, self.capacity_hint)
@@ -1437,16 +1494,25 @@ class DevGroupbyReduce(DevFn):
     what the ranks send in rank order -- and on a NaN partial meaning "no value in that partition", exactly as a NaN
     row does (under ``skipna=False`` every column takes the group's first / last partial row)."""
 
-    def __init__(self, agg: str, skipna: bool = True):
+    def __init__(self, agg: str, skipna: bool = True, nan_key: bool = False):
         self.agg = agg
         self.op = f"groupby_{agg}_reduce"
         self.skipna = skipna
+        self.nan_key = nan_key
 
     def _merge(self, keys, cols):
         """Regroup partial rows by key -> ascending unique keys + merged partial columns (same layout as the input).
         Partial sums add up, partial minima / maxima reduce with min / max, counts and sizes add up."""
         if self.agg in _POSITION_AGGS:
             return _first_last(self.agg, keys, list(cols), self.skipna, len(keys))
+        if self.agg in _ARG_AGGS:
+            # the same two-pass table over the partial VALUES, whose positions are partial rows: the earlier partition
+            # (or rank) wins a tie, and a NaN partial -- no value in that partition -- is skipped like a NaN row
+            W = len(cols) // 2
+            k, pos = _arg_positions(self.agg, keys, cols[:W], len(keys))
+            return k, [ops.take_columns([c], p)[0] for c, p in zip(cols[:W], pos)] + [
+                ops.take_columns([c], p)[0] for c, p in zip(cols[W:], pos)]  # fmt: skip
+
         layout = _PARTIALS[self.agg]
         W = len(cols) // len(layout.arrays)
         got = {name: list(cols[i * W : (i + 1) * W]) for i, name in enumerate(layout.arrays)}
@@ -1458,8 +1524,34 @@ class DevGroupbyReduce(DevFn):
         return k, _partial_cols(self.agg, s, c, z)
 
     def _finalize(self, k, cols, columns, key_label):
+        if self.agg in _ARG_AGGS:
+            W = len(cols) // 2
+            return _group_block(cols[W:], pandas.Index([t[1] for t in columns[W:]]), k, key_label)
         labels = pandas.Index([t[1] for t in columns[: len(cols) // 2]]) if self.agg == "mean" else columns
         return _finished_block(self.agg, k, key_label, cols, labels)
+
+    def _refuse_all_na(self, k, cols, spans: bool):
+        """pandas' ValueError when a group of the result has no non-NaN value in some column: its merged value is
+        NaN.  The NaN group of a float key (image INT64_MAX, the last key) does not reach the result under
+        ``dropna`` (``nan_key``), so it does not count.  Across ranks the decision is job-wide: one host integer per
+        rank, combined before anybody raises."""
+        W = len(cols) // 2
+        floats = [c for c in cols[:W] if c.dtype == np.float64]
+        n = len(k)
+        if floats and n and self.nan_key and int(k.data[n - 1].item()) == (1 << 63) - 1:
+            n -= 1
+            floats = [DeviceColumn(c.data[:n], c.dtype) for c in floats]
+        missing = 0
+        if floats and n:
+            t = ops.torch_mod()
+            _, cnts = ops.reduce_columns("count", floats)
+            missing = sum(n - c for c in t.cat([c.reshape(1) for c in cnts]).tolist())  # one D2H
+        if spans:
+            from . import dist
+
+            missing = dist.control_sum(missing)
+        if missing:
+            raise ValueError(f"{self.agg} with skipna=True encountered all NA values in a group.")
 
     def __call__(self, block, *args, partition_idx=0, **kwargs):
         _check_block(block, self.op)
@@ -1469,8 +1561,11 @@ class DevGroupbyReduce(DevFn):
         # a single partial table (one row partition on this GPU) is already one row per key, ascending:
         # nothing to regroup -- the reference would re-run groupby(level=0) on it to the same effect
         k, cols = (keys, list(block.cols)) if block.keys_sorted_unique else self._merge(keys, block.cols)
-        if _spans_ranks(block):
+        spans = _spans_ranks(block)
+        if spans:
             k, cols = self._across_ranks(k, cols)
+        if self.agg in _ARG_AGGS:
+            self._refuse_all_na(k, cols, spans)
         return self._finalize(k, cols, block.columns, key_label)
 
     def _across_ranks(self, k, cols):
@@ -1502,9 +1597,9 @@ def fused_dense_groupby(map_fn: "DevGroupbyMap", reduce_fn: "DevGroupbyReduce", 
     agg = map_fn.agg
     if agg != reduce_fn.agg or not blocks or len(blocks) != len(by_blocks):
         return None
-    if agg in _POSITION_AGGS:
+    if agg in _POSITION_AGGS or agg in _ARG_AGGS:
         # merging position tables across GPUs would need the values gathered across GPUs too: the general path
-        # (still one dense table per partition when the key range allows) does first / last
+        # (still one dense table per partition when the key range allows) does first / last / idxmax / idxmin
         return None
     inputs = [_split_key_values(block, by_block, map_fn.op) for block, by_block in zip(blocks, by_blocks)]
     key_label, labels = inputs[0][1], (inputs[0][3] if agg != "size" else inputs[0][3][:0])

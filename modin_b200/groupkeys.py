@@ -149,7 +149,7 @@ def restore_keys(blocks: List[DeviceBlock], image, dropna: bool = True, names=No
 
 
 # ---- dictionary aggregation --------------------------------------------------------------------------------------
-_DICT_AGGS = ("sum", "count", "mean", "min", "max", "first", "last")
+_DICT_AGGS = ("sum", "count", "mean", "min", "max", "first", "last", "idxmax", "idxmin")
 
 
 def split_aggregations(spec: dict, columns, keys=()) -> Dict[str, list]:
@@ -174,8 +174,9 @@ def zip_aggregations(spec: dict, by_func: Dict[str, list], results: List[List[li
     if any(len(row) != 1 for rows in results for row in rows):
         raise NotImplementedError("dictionary aggregation over more than 32 columns per function")
     if len({tuple(row[0].nrows for row in rows) for rows in results}) != 1 and not dist.is_distributed():
-        # first / last never take the fused one-table path, so next to another function their results can be split
-        # into row partitions differently; each holds every group once, ascending, so one block per result lines up
+        # first / last / idxmax / idxmin never take the fused one-table path, so next to another function their results
+        # can be split into row partitions differently; each holds every group once, ascending, so one block per result
+        # lines up
         results = [[[concat_rows([row[0] for row in rows])]] for rows in results]
     if len({len(rows) for rows in results}) != 1:
         raise NotImplementedError("per-function results are partitioned differently")

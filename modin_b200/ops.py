@@ -255,8 +255,10 @@ def arg_reduce_columns(op: str, cols: Sequence[DeviceColumn], variant: int = 0):
 
 
 # ------------------------------------------------------------------ GroupByReduce
-_GB_POS = _lib.GB_FIRST | _lib.GB_LAST  # tables of int64 row positions (first / last)
+_GB_ARG = _lib.GB_ARGMIN | _lib.GB_ARGMAX  # idxmin / idxmax: extreme images in ``cnt``, row positions in ``acc``
+_GB_POS = _lib.GB_FIRST | _lib.GB_LAST | _GB_ARG  # tables of int64 row positions (first / last / idxmin / idxmax)
 _GB_ACC = _lib.GB_SUM | _lib.GB_MIN | _lib.GB_MAX | _GB_POS
+_GB_CNT = _lib.GB_COUNT | _GB_ARG  # tables with a ``cnt`` array
 _DENSE_ARRAYS = ("acc", "cnt", "size", "present")
 
 
@@ -298,7 +300,7 @@ class GroupTable:
         arrays = {}
         if flags & _GB_ACC:
             arrays["acc"] = t.empty(R * vs, dtype=t.float64 if flags & _lib.GB_SUM else t.int64, device=dev)
-        if flags & _lib.GB_COUNT:
+        if flags & _GB_CNT:
             arrays["cnt"] = t.empty(R * vs, dtype=t.int64, device=dev)
         if flags & _lib.GB_SIZE:
             arrays["size"] = t.empty(R, dtype=t.int64, device=dev)
@@ -354,9 +356,19 @@ class GroupTable:
 
     def accumulate(self, keys: DeviceColumn, vals: Sequence[Optional[DeviceColumn]]):
         """Aggregate rows ``keys`` / ``vals`` (float64 columns).  A first / last table also takes None for a column
-        without NaN: every row of it counts.  Positions run on across calls, in call order."""
+        without NaN: every row of it counts.  Positions run on across calls, in call order.  An idxmin / idxmax table
+        takes float64 and int64 columns, in ONE call (mb200_gb_accumulate_arg): its positions are that call's rows."""
         if keys.dtype != np.int64:
             raise TypeError("device groupby needs an int64 key column")
+        if self.flags & _GB_ARG:
+            if any(v is None or v.dtype not in (np.float64, np.int64) for v in vals):
+                raise TypeError("device groupby.idxmax / idxmin take float64 and int64 value columns")
+            mask = sum(1 << j for j, v in enumerate(vals) if v.dtype == np.int64)
+            ptrs = _lib.ptr_array([v.ptr for v in vals])
+            with _timed("gb_accumulate_arg"):
+                _lib.check(self.lib.mb200_gb_accumulate_arg(self.handle, keys.ptr, ptrs, mask, len(keys),
+                                                            current_stream()))  # fmt: skip
+            return
         for v in vals:
             if v is None and self.flags & _GB_POS:
                 continue
@@ -382,7 +394,7 @@ class GroupTable:
 
     def _outputs(self, rows: int):
         """Empty (keys, sums, cnts, sizes) columns of ``rows`` rows for what this table emits."""
-        acc_dtype = np.int64 if self.flags & _GB_POS else np.float64  # first / last emit row positions
+        acc_dtype = np.int64 if self.flags & _GB_POS else np.float64  # first / last / idxmin / idxmax emit row positions
         sums = [DeviceColumn.empty(rows, acc_dtype) for _ in range(self.nvals)] if self.flags & _GB_ACC else None
         cnts = [DeviceColumn.empty(rows, np.int64) for _ in range(self.nvals)] if self.flags & _lib.GB_COUNT else None
         sizes = DeviceColumn.empty(rows, np.int64) if self.flags & _lib.GB_SIZE else None
@@ -526,7 +538,7 @@ def dense_range_ok(lo: int, hi: int, cap: int, total_rows: int, nvals: int, flag
     rng = hi - lo + 1
     if rng > (1 << 29) or rng > max(4 * cap, total_rows // 2, 1 << 16):
         return False
-    arrays = (1 if flags & _GB_ACC else 0) + (1 if flags & _lib.GB_COUNT else 0)
+    arrays = (1 if flags & _GB_ACC else 0) + (1 if flags & _GB_CNT else 0)
     return rng * (value_stride(nvals) * 8 * arrays + 9) <= DENSE_TABLE_MAX_BYTES
 
 

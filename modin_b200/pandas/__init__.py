@@ -625,12 +625,23 @@ class DataFrameGroupBy:
         return self._wrap_aggregation(type(self._query_compiler).groupby_last, numeric_only,
                                       agg_kwargs=dict(min_count=min_count, skipna=skipna))  # fmt: skip
 
+    def idxmax(self, skipna=True, numeric_only=False):
+        """The label of the first row holding each group's maximum, per column (NaN skipped; a group whose values in a
+        column are all NaN raises ValueError), passed on as modin/pandas/groupby.py:607-618 does."""
+        return self._wrap_aggregation(type(self._query_compiler).groupby_idxmax, numeric_only,
+                                      agg_kwargs=dict(axis=0, skipna=skipna))  # fmt: skip
+
+    def idxmin(self, skipna=True, numeric_only=False):
+        return self._wrap_aggregation(type(self._query_compiler).groupby_idxmin, numeric_only,
+                                      agg_kwargs=dict(axis=0, skipna=skipna))  # fmt: skip
+
     def size(self):
         res = self._wrap_aggregation(type(self._query_compiler).groupby_size)
         return Series(query_compiler=res._query_compiler)
 
     def agg(self, func, *args, **kwargs):
-        if isinstance(func, str) and func in ("sum", "count", "mean", "size", "min", "max", "first", "last"):
+        if isinstance(func, str) and func in ("sum", "count", "mean", "size", "min", "max", "first", "last", "idxmax",
+                                                 "idxmin"):
             return getattr(self, func)()
         if isinstance(func, dict):
             return self._dict_agg(func)

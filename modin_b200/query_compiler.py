@@ -28,6 +28,7 @@ from . import groupkeys as gk
 from .block import concat_cols
 from .dataframe import B200Dataframe
 from .functors import (
+    arg_label_dtype,
     DevArgReduce,
     DevAstype,
     DevBinary,
@@ -67,10 +68,28 @@ def _position_agg_skipna(agg: str, agg_kwargs) -> bool:
     return bool(skipna)
 
 
+def _arg_agg_kwargs(agg: str, agg_kwargs) -> None:
+    """``groupby.idxmax`` / ``idxmin`` take ``skipna=True`` and ``axis=0`` from the ``agg_kwargs`` Modin passes
+    (modin/pandas/groupby.py:607-631).  ``skipna=False`` is refused: pandas 3.0.2 raises there when a NaN is present
+    anywhere, even in a row whose key is dropped, and otherwise returns NaN for every group."""
+    kw = dict(agg_kwargs or {})
+    skipna, axis = kw.pop("skipna", True), kw.pop("axis", 0)
+    kw.pop("numeric_only", None)
+    if kw:
+        raise NotImplementedError(f"groupby.{agg}({', '.join(kw)}=) is not on the B200 path")
+    if not isinstance(skipna, (bool, np.bool_)):
+        raise ValueError(f"skipna must be a boolean, got {skipna!r}")
+    if not skipna:
+        raise NotImplementedError(f"groupby.{agg}(skipna=False) is not on the B200 path")
+    if axis not in (0, "index", None):
+        raise NotImplementedError(f"groupby.{agg}(axis={axis!r}) is not on the B200 path")
+
+
 def _groupby_reduce(agg: str):
     """``qc.groupby_<agg>`` (qc.py:3741-3748, alg/groupby.py) over device blocks.  ``by`` is a query compiler of key
     columns with the frame's rows; ``key_names`` replaces the names of the result's keys (``groupby(level=)``).
-    ``agg_kwargs`` are read by first / last only (``skipna``, ``min_count``); the other aggregations ignore them."""
+    ``agg_kwargs`` are read by first / last (``skipna``, ``min_count``) and idxmax / idxmin (``skipna``, ``axis``) only;
+    the other aggregations ignore them."""
     map_f, red_f = DevGroupbyMap(agg), DevGroupbyReduce(agg)
 
     def caller(query_compiler, by, axis, groupby_kwargs, agg_args, agg_kwargs, drop=False, key_names=None, **kwargs):
@@ -84,6 +103,8 @@ def _groupby_reduce(agg: str):
         if agg in ("first", "last"):
             skipna = _position_agg_skipna(agg, agg_kwargs)
             fns = (DevGroupbyMap(agg, skipna=skipna), DevGroupbyReduce(agg, skipna=skipna))
+        if agg in ("idxmax", "idxmin"):
+            _arg_agg_kwargs(agg, agg_kwargs)
         frame, by_frame = query_compiler._modin_frame, by._modin_frame
         # a float64 key or several int64 keys: the single-key groupby runs on their int64 image and the G result keys
         # are restored afterwards (groupkeys.py); one int64 key is its own image
@@ -96,6 +117,12 @@ def _groupby_reduce(agg: str):
         if drop and len(by.columns) > 1:  # the packed key has a label of its own: the key columns leave here
             keep = [c for c in query_compiler.columns if c not in set(by.columns)]
             frame = query_compiler.getitem_column_array(keep)._modin_frame
+        if agg in ("idxmax", "idxmin"):
+            # labels of one dtype on every rank; the NaN group of a float key is dropped below under dropna, so it is
+            # left out of the all-NaN check
+            labels = arg_label_dtype([row[0].get() for row in frame._partitions])
+            nan_key = image == gk.FLOAT_KEY and groupby_kwargs.get("dropna", True)
+            fns = (DevGroupbyMap(agg, label_dtype=labels), DevGroupbyReduce(agg, nan_key=nan_key))
         # the functors themselves, not lambdas around them: the partition manager recognises them and fuses map +
         # reduce into one direct-addressed table per GPU when the key range allows (pm.groupby_reduce)
         new_frame = frame.groupby_reduce(axis, by_frame, *fns)
@@ -210,8 +237,10 @@ def device_operations(alg):
         groupby_max = _groupby_reduce("max")
         groupby_first = _groupby_reduce("first")
         groupby_last = _groupby_reduce("last")
+        groupby_idxmax = _groupby_reduce("idxmax")
+        groupby_idxmin = _groupby_reduce("idxmin")
 
-        _DEVICE_AGGS = ("sum", "count", "size", "mean", "min", "max", "first", "last")
+        _DEVICE_AGGS = ("sum", "count", "size", "mean", "min", "max", "first", "last", "idxmax", "idxmin")
 
         def groupby_agg(self, by, agg_func, axis, groupby_kwargs, agg_args, agg_kwargs, how="axis_wise", drop=False,
                         series_groupby=False):  # fmt: skip
@@ -222,7 +251,7 @@ def device_operations(alg):
             ask for it; every result carries the same ascending group keys, so the result blocks are zipped
             column-wise (buffers shared) in the dictionary's order.  A function name alone goes to its registered
             template.  Anything else has no device form and is refused -- there is no pandas block to fall back to."""
-            if how != "axis_wise" or agg_args or (agg_kwargs and agg_func not in ("first", "last")):
+            if how != "axis_wise" or agg_args or (agg_kwargs and agg_func not in ("first", "last", "idxmax", "idxmin")):
                 raise NotImplementedError(f"groupby ({how}) with extra arguments is not on the B200 path")
             if isinstance(agg_func, str) and agg_func in self._DEVICE_AGGS:
                 return getattr(self, f"groupby_{agg_func}")(
@@ -234,10 +263,11 @@ def device_operations(alg):
                 raise NotImplementedError("device groupby: key columns of the same frame, axis=0")
             spec = {col: fn[0] if isinstance(fn, (list, tuple)) and len(fn) == 1 else fn for col, fn in agg_func.items()}
             by_func = gk.split_aggregations(spec, self.columns, set(by.columns) if drop else ())
-            if len(by_func) > 1 and set(by_func) & {"first", "last"} and dist.is_distributed():
-                # across ranks the fused dense path of the other functions and the key-range exchange of first / last
-                # give each rank a different key range
-                raise NotImplementedError("groupby.agg mixing first / last with other functions across ranks")
+            if len(by_func) > 1 and set(by_func) & {"first", "last", "idxmax", "idxmin"} and dist.is_distributed():
+                # across ranks the fused dense path of the other functions and the key-range exchange of first / last /
+                # idxmax / idxmin give each rank a different key range
+                raise NotImplementedError("groupby.agg mixing first / last / idxmax / idxmin with other functions "
+                                          "across ranks")  # fmt: skip
             if any(isinstance(fn, (list, tuple)) for fn in agg_func.values()):
                 raise NotImplementedError("groupby.agg with lists of functions (two-level result columns)")
             kw = dict(groupby_kwargs, as_index=True)
