@@ -23,7 +23,7 @@
 //     256-row tiles of the key + value columns into a shared-memory ring with 1-D TMA bulk copies
 //     (full/empty mbarriers), so DRAM latency is out of the per-row dependency chain and no
 //     registers hold in-flight rows; 8 consumer warps each take 32 rows of a tile.
-//   gb_accumulate_kernel (ragged tails, unaligned views, V > 8, partial-table merges, or MB200_GB_VARIANT):
+//   gb_accumulate_kernel (ragged tails, unaligned views, V > 8, partial-table merges, or MB200_GB_VARIANT=1):
 //     the same per-warp algorithm with direct coalesced loads and 40 resident warps per SM.
 // Per warp (32 rows):
 //   1. warp-cooperative probe: __match_any_sync groups lanes holding the same key; the lowest lane
@@ -125,38 +125,19 @@ struct GbParams {
   int dense;              // direct-addressed table: gid = key - kbase
   long long kbase;
   unsigned int* present;  // dense: one byte per key of [kbase, kbase + gcap)
-  int policy_mode;  // unused (kept for experiments)
-  int prefetch;     // TMA kernel: L2-prefetch the next tile's probe slots (MB200_GB_PREFETCH=0 disables)
 };
 
-// ---- table accesses: relaxed GPU-scope, plain forms; `pol` (an explicit L2 eviction priority via
-// createpolicy + .L2::cache_hint) is kept in the signatures for experiments.
-__device__ __forceinline__ void red_add_f64(double* p, double v, uint64_t pol) {
-  if (pol)  // experiment (MB200_GB_POLICY): explicit L2 eviction priority on the accumulator updates
-    asm volatile("red.relaxed.gpu.global.add.L2::cache_hint.f64 [%0], %1, %2;" ::"l"(p), "d"(v), "l"(pol) : "memory");
-  else
-    asm volatile("red.relaxed.gpu.global.add.f64 [%0], %1;" ::"l"(p), "d"(v) : "memory");
+// ---- table accesses: relaxed GPU-scope
+__device__ __forceinline__ void red_add_f64(double* p, double v) {
+  asm volatile("red.relaxed.gpu.global.add.f64 [%0], %1;" ::"l"(p), "d"(v) : "memory");
 }
-__device__ __forceinline__ void red_add_u64(long long* p, long long v, uint64_t) {
+__device__ __forceinline__ void red_add_u64(long long* p, long long v) {
   asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
-__device__ __forceinline__ void ld_slot(const Slot* s, long long& key, int& gid, uint64_t) {
-  unsigned long long a, b;
-  asm volatile("ld.relaxed.gpu.global.v2.u64 {%0,%1}, [%2];" : "=l"(a), "=l"(b) : "l"(s) : "memory");
-  key = (long long)a;
-  gid = (int)(unsigned int)(b & 0xffffffffULL);
-}
-__device__ __forceinline__ void st_slot(Slot* s, long long key, int gid, uint64_t) {
+__device__ __forceinline__ void st_slot(Slot* s, long long key, int gid) {
   const unsigned long long b = (unsigned long long)(unsigned int)gid;
   asm volatile("st.relaxed.gpu.global.v2.u64 [%0], {%1,%2};" ::"l"(s), "l"((unsigned long long)key), "l"(b)
                : "memory");
-}
-__device__ __forceinline__ uint64_t table_policy(int mode) {
-  uint64_t pol = 0;
-  if (mode == 1) asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
-  if (mode == 2) asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(pol));
-  if (mode == 3) asm volatile("createpolicy.fractional.L2::evict_unchanged.b64 %0, 1.0;" : "=l"(pol));
-  return pol;
 }
 
 // min / max accumulators share the `acc` array: doubles are stored through an order-preserving map to
@@ -177,8 +158,8 @@ __device__ __forceinline__ void red_max_s64(long long* p, long long v) {
   asm volatile("red.relaxed.gpu.global.max.s64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 // value accumulator update of one (group, column): sum, or min / max on the ordered image
-__device__ __forceinline__ void acc_update(const GbParams& p, size_t o, double xv, uint64_t keep) {
-  if (p.flags & MB200_GB_SUM) red_add_f64(p.acc + o, xv, keep);
+__device__ __forceinline__ void acc_update(const GbParams& p, size_t o, double xv) {
+  if (p.flags & MB200_GB_SUM) red_add_f64(p.acc + o, xv);
   else if (p.flags & MB200_GB_MIN) red_min_s64(reinterpret_cast<long long*>(p.acc) + o, f64_to_ordered(xv));
   else if (p.flags & MB200_GB_MAX) red_max_s64(reinterpret_cast<long long*>(p.acc) + o, f64_to_ordered(xv));
 }
@@ -309,7 +290,7 @@ __device__ __noinline__ int insert_rounds(const GbParams& p, long long k, bool i
           p.meta->overflow = 1;
           ng = gcap;
         }
-        st_slot(&p.slots[2 * (size_t)bucket + sub], k, ng, 0);
+        st_slot(&p.slots[2 * (size_t)bucket + sub], k, ng);
         gid = ng;
       }
     }
@@ -318,7 +299,7 @@ __device__ __noinline__ int insert_rounds(const GbParams& p, long long k, bool i
 }
 
 // Dense group id of every lane's key (gcap = table overflowed).  Must be called by all 32 lanes.
-__device__ __forceinline__ int resolve_gid(const GbParams& p, long long k, uint64_t) {
+__device__ __forceinline__ int resolve_gid(const GbParams& p, long long k) {
   if (p.dense) {
     // direct addressing (kernel-uniform branch): no probe, no slots, and normally no presence access either:
     // dense accumulators start from a value no update can leave behind (-0.0 for sums, the "no value yet"
@@ -345,7 +326,7 @@ __device__ __forceinline__ int resolve_gid(const GbParams& p, long long k, uint6
 // ---------------------------------------------------------------- fallback: direct loads
 // POS: FIRST / LAST tables (raw rows only) -- positions go to the accumulators, and a NULL value column reads as
 // "no NaN" without a load.  POS = false compiles to the code these kernels had before FIRST / LAST existed.
-template <int VARIANT, bool PARTIAL, bool POS>
+template <bool PARTIAL, bool POS>
 __global__ void __launch_bounds__(kGbThreads, 5) gb_accumulate_kernel(const __grid_constant__ GbParams p) {
   static_assert(!(POS && PARTIAL), "FIRST / LAST tables take raw rows only");
   __shared__ double s_tile[kGbWarps][8 * kColStride];
@@ -354,7 +335,6 @@ __global__ void __launch_bounds__(kGbThreads, 5) gb_accumulate_kernel(const __gr
   const long long wstride = (long long)gridDim.x * kGbWarps;
   const int gcap = (int)p.gcap;
   const uint64_t pol = l2_policy_evict_first();
-  const uint64_t keep = table_policy(p.policy_mode);
   for (long long ch = (long long)blockIdx.x * kGbWarps + warp; ch < nchunks; ch += wstride) {
     const long long base = ch << 5;
     const long long row = base + lane;
@@ -375,10 +355,10 @@ __global__ void __launch_bounds__(kGbThreads, 5) gb_accumulate_kernel(const __gr
       const long long k0 = __shfl_sync(0xffffffffu, k, 0);
       k = valid ? k : k0;
     }
-    const int gid = resolve_gid(p, k, keep);
+    const int gid = resolve_gid(p, k);
     const bool live = valid && gid < gcap;
 
-    if ((p.flags & MB200_GB_SIZE) && live) red_add_u64(p.size + gid, PARTIAL ? p.psize[row] : 1LL, keep);
+    if ((p.flags & MB200_GB_SIZE) && live) red_add_u64(p.size + gid, PARTIAL ? p.psize[row] : 1LL);
     if (p.dense && p.nvals == 0 && !(p.flags & MB200_GB_SIZE) && live) dense_mark(p, gid);  // keys only
     // ---- accumulate, 8 value columns at a time
     for (int c0 = 0; c0 < p.nvals; c0 += 8) {
@@ -390,68 +370,47 @@ __global__ void __launch_bounds__(kGbThreads, 5) gb_accumulate_kernel(const __gr
                      ? ldg_stream_f64(static_cast<const double*>(p.vals[c0 + c]) + row, pol)
                      : 0.0;
       }
-      if (VARIANT == 1) {  // lane == row (kept for measurement)
-        bool rowvis = false;
+      double* tile = s_tile[warp];
 #pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          if (c < nc && live) {
-            const size_t o = (size_t)gid * p.vstride + c0 + c;
-            rowvis = rowvis || (!PARTIAL && dense_visible<POS>(p, x[c]));
-            if (POS) {
-              if (x[c] == x[c]) pos_update(p, o, p.row0 + row);
-            } else if (x[c] == x[c]) {
-              acc_update(p, o, x[c], keep);
-            }
-            if (p.flags & MB200_GB_COUNT) {
-              if (PARTIAL) red_add_u64(p.cnt + o, static_cast<const long long*>(p.pcnt[c0 + c])[row], keep);
-              else if (x[c] == x[c]) red_add_u64(p.cnt + o, 1LL, keep);
-            }
+      for (int c = 0; c < 8; ++c) tile[c * kColStride + lane] = x[c];
+      __syncwarp();
+      const int c = lane & 7;
+      unsigned int seen = 0, rowok = 0;
+      int gs[8];
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        const int r = 4 * kk + (lane >> 3);
+        const int g = __shfl_sync(0xffffffffu, gid, r);
+        const double xv = tile[c * kColStride + r];
+        const bool ok = (base + r < p.nrows) && (c < nc) && (g < gcap);
+        gs[kk] = g;
+        if ((base + r < p.nrows) && g < gcap) rowok |= 1u << kk;
+        if (ok) {
+          const size_t o = (size_t)g * p.vstride + c0 + c;
+          if (!PARTIAL && dense_visible<POS>(p, xv)) seen |= 1u << kk;
+          if (POS) {
+            if (xv == xv) pos_update(p, o, p.row0 + base + r);
+          } else if (xv == xv) {
+            acc_update(p, o, xv);
+          }
+          if (p.flags & MB200_GB_COUNT) {
+            if (PARTIAL) red_add_u64(p.cnt + o, static_cast<const long long*>(p.pcnt[c0 + c])[base + r]);
+            else if (xv == xv) red_add_u64(p.cnt + o, 1LL);
           }
         }
-        if (p.dense && !(p.flags & MB200_GB_SIZE) && live && !rowvis) dense_mark(p, gid);
-      } else {
-        double* tile = s_tile[warp];
-#pragma unroll
-        for (int c = 0; c < 8; ++c) tile[c * kColStride + lane] = x[c];
-        __syncwarp();
-        const int c = lane & 7;
-        unsigned int seen = 0, rowok = 0;
-        int gs[8];
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          const int r = 4 * kk + (lane >> 3);
-          const int g = __shfl_sync(0xffffffffu, gid, r);
-          const double xv = tile[c * kColStride + r];
-          const bool ok = (base + r < p.nrows) && (c < nc) && (g < gcap);
-          gs[kk] = g;
-          if ((base + r < p.nrows) && g < gcap) rowok |= 1u << kk;
-          if (ok) {
-            const size_t o = (size_t)g * p.vstride + c0 + c;
-            if (!PARTIAL && dense_visible<POS>(p, xv)) seen |= 1u << kk;
-            if (POS) {
-              if (xv == xv) pos_update(p, o, p.row0 + base + r);
-            } else if (xv == xv) {
-              acc_update(p, o, xv, keep);
-            }
-            if (p.flags & MB200_GB_COUNT) {
-              if (PARTIAL) red_add_u64(p.cnt + o, static_cast<const long long*>(p.pcnt[c0 + c])[base + r], keep);
-              else if (xv == xv) red_add_u64(p.cnt + o, 1LL, keep);
-            }
-          }
-        }
-        if (p.dense && !(p.flags & MB200_GB_SIZE)) {  // rows that left no trace mark their presence byte
-          seen |= __shfl_xor_sync(0xffffffffu, seen, 1);
-          seen |= __shfl_xor_sync(0xffffffffu, seen, 2);
-          seen |= __shfl_xor_sync(0xffffffffu, seen, 4);
-          const unsigned int unseen = ~seen & rowok;
-          if (c == 0 && unseen) {
-#pragma unroll
-            for (int kk = 0; kk < 8; ++kk)
-              if ((unseen >> kk) & 1u) dense_mark(p, gs[kk]);
-          }
-        }
-        __syncwarp();
       }
+      if (p.dense && !(p.flags & MB200_GB_SIZE)) {  // rows that left no trace mark their presence byte
+        seen |= __shfl_xor_sync(0xffffffffu, seen, 1);
+        seen |= __shfl_xor_sync(0xffffffffu, seen, 2);
+        seen |= __shfl_xor_sync(0xffffffffu, seen, 4);
+        const unsigned int unseen = ~seen & rowok;
+        if (c == 0 && unseen) {
+#pragma unroll
+          for (int kk = 0; kk < 8; ++kk)
+            if ((unseen >> kk) & 1u) dense_mark(p, gs[kk]);
+        }
+      }
+      __syncwarp();
     }
   }
 }
@@ -533,7 +492,6 @@ __global__ void __launch_bounds__(kGbTmaThreads) gb_accumulate_tma_kernel(const 
     return;
   }
   // ---------------- consumers: warp w owns rows [32w, 32w + 32) of every tile
-  const uint64_t keep = table_policy(p.policy_mode);
   const int c = lane & 7;
   const bool nullcol = POS && c < nv && !p.vals[c];  // POS: this lane's column has no NaN and no staged tile
   for (long long k = 0; k < nmine; ++k) {
@@ -541,18 +499,8 @@ __global__ void __launch_bounds__(kGbTmaThreads) gb_accumulate_tma_kernel(const 
     mbar_wait(&full[s], (uint32_t)((k / STAGES) & 1));
     const double* stage = reinterpret_cast<const double*>(smem_raw + (size_t)s * kStageBytes);
     const long long key = reinterpret_cast<const long long*>(stage)[warp * 32 + lane];
-    if (p.prefetch && k + 1 < nmine) {
-      // the next tile's keys are (normally) already in shared memory: pull the first probe slot of each of
-      // this warp's next 32 rows into L2 now, one tile ahead of the dependent 128-bit slot load
-      const int s1 = (int)((k + 1) % STAGES);
-      mbar_wait(&full[s1], (uint32_t)(((k + 1) / STAGES) & 1));
-      const long long nk =
-          reinterpret_cast<const long long*>(smem_raw + (size_t)s1 * kStageBytes)[warp * 32 + lane];
-      const Slot* ns = &p.slots[hash_key(nk) & p.mask];
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(ns));
-    }
-    int gid = resolve_gid(p, key, keep);
-    if ((p.flags & MB200_GB_SIZE) && gid < gcap) red_add_u64(p.size + gid, 1LL, keep);
+    int gid = resolve_gid(p, key);
+    if ((p.flags & MB200_GB_SIZE) && gid < gcap) red_add_u64(p.size + gid, 1LL);
     if (HOT && gid < gcap) {  // is this row's group in the CTA's hot cache (or can it claim its slot)?
       const int slot = gid & (kHotSlots - 1);
       int tag = *reinterpret_cast<volatile int*>(&s_tag[slot]);
@@ -583,8 +531,8 @@ __global__ void __launch_bounds__(kGbTmaThreads) gb_accumulate_tma_kernel(const 
             if (p.flags & MB200_GB_COUNT) atomicAdd(&s_hcnt[o], 1u);
           } else {
             const size_t o = (size_t)g * p.vstride + c;
-            acc_update(p, o, xv, keep);
-            if (p.flags & MB200_GB_COUNT) red_add_u64(p.cnt + o, 1LL, keep);
+            acc_update(p, o, xv);
+            if (p.flags & MB200_GB_COUNT) red_add_u64(p.cnt + o, 1LL);
           }
         }
       }
@@ -613,9 +561,9 @@ __global__ void __launch_bounds__(kGbTmaThreads) gb_accumulate_tma_kernel(const 
       const int tag = s_tag[slot];
       if (tag < 0 || cc >= nv) continue;
       const size_t o = (size_t)tag * p.vstride + cc;
-      if (p.flags & MB200_GB_SUM) red_add_f64(p.acc + o, s_hot[slot * kHotStride + cc], 0);
+      if (p.flags & MB200_GB_SUM) red_add_f64(p.acc + o, s_hot[slot * kHotStride + cc]);
       if ((p.flags & MB200_GB_COUNT) && s_hcnt[slot * kHotStride + cc])
-        red_add_u64(p.cnt + o, (long long)s_hcnt[slot * kHotStride + cc], 0);
+        red_add_u64(p.cnt + o, (long long)s_hcnt[slot * kHotStride + cc]);
     }
   }
 }
@@ -718,7 +666,7 @@ __global__ void __launch_bounds__(kSmemThreads, 1) gb_accumulate_smem_kernel(con
     if (f_sum) {
       double a = s_acc[o];
       for (int r = 1; r < nrep; ++r) a += s_acc[r * rstride + o];
-      red_add_f64(p.acc + i, a, 0);
+      red_add_f64(p.acc + i, a);
     } else if (f_min || f_max) {
       long long a = s_acc_i[o];
       for (int r = 1; r < nrep; ++r) {
@@ -731,7 +679,7 @@ __global__ void __launch_bounds__(kSmemThreads, 1) gb_accumulate_smem_kernel(con
     if (f_cnt) {
       long long n = 0;
       for (int r = 0; r < nrep; ++r) n += s_cnt[r * rstride + o];
-      if (n) red_add_u64(p.cnt + i, n, 0);
+      if (n) red_add_u64(p.cnt + i, n);
     }
   }
   for (int g = tid; g < R; g += kSmemThreads) {
@@ -740,7 +688,7 @@ __global__ void __launch_bounds__(kSmemThreads, 1) gb_accumulate_smem_kernel(con
     if (f_size) {
       long long n = 0;
       for (int r = 0; r < nrep; ++r) n += s_size[r * zstride + g];
-      red_add_u64(p.size + g, n, 0);
+      red_add_u64(p.size + g, n);
     }
   }
 }
@@ -1000,40 +948,30 @@ static long long next_pow2(long long v) {
   return p;
 }
 
-// MB200_GB_VARIANT: 0 = TMA-staged tiles, 1 = direct loads + 8-lanes-per-row REDs, 2 = direct loads +
-// lane == row REDs; unset = the TMA-staged kernel.  Read per call so one process can compare them.
-// Measured on an H100 80GB HBM3 (400 W power limit), 2^27 rows, V = 8, fresh table per pass, uniform keys, ms for
-// variants 0 / 1 / 2: G = 65536 dense 5.3 / 6.1 / 13.5, hashed 6.4 / 7.2 / 14.6; G = 1e6 (64 MB dense, 96 MB hashed:
-// both larger than the 50 MB L2) dense 13.6 / 13.4 / 21.6, hashed 21.5 / 21.9 / 30.4.  With skewed keys only the TMA
-// kernel has the hot-group cache (6.1 ms against 81 and 246 at G = 1e6).  So the TMA kernel is taken at every size.
-static int gb_variant_from_env(size_t table_bytes, size_t l2_bytes) {
-  const char* e = getenv("MB200_GB_VARIANT");
-  if (e && e[0] == '0') return 0;
-  if (e && e[0] == '1') return 1;
-  if (e && e[0] == '2') return 2;
-  (void)table_bytes;
-  (void)l2_bytes;
-  return 0;
+// The arrays a table of these flags has, and the int64 word each starts from ("no value yet").
+//   acc: float64 sums, min / max as order-preserving images, or FIRST / LAST / ARG row positions.  Dense sums start
+//        from -0.0, the one value no sum can end on (x + -0.0 = x, and the emit turns it into +0.0), so that a key whose
+//        accumulators moved is present; hashed sums from 0.  Min, FIRST and ARG positions start from INT64_MAX, max and
+//        LAST from INT64_MIN.
+//   cnt: non-NaN counts from 0, or an ARG table's extreme images: from INT64_MIN for ARGMAX, INT64_MAX for ARGMIN.
+//   size: rows per group, from 0.
+struct TableArrays {
+  bool acc, cnt, size;
+  long long acc_init, cnt_init;
+};
+static TableArrays table_arrays(int flags, bool dense) {
+  const long long lo = (long long)0x8000000000000000ULL, hi = 0x7fffffffffffffffLL;
+  TableArrays a;
+  a.acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST | kGbArg);
+  a.cnt = flags & (MB200_GB_COUNT | kGbArg);
+  a.size = flags & MB200_GB_SIZE;
+  a.acc_init = (flags & MB200_GB_SUM) ? (dense ? lo : 0) : (flags & (MB200_GB_MIN | MB200_GB_FIRST | kGbArg)) ? hi : lo;
+  a.cnt_init = (flags & MB200_GB_ARGMAX) ? lo : (flags & MB200_GB_ARGMIN) ? hi : 0;
+  return a;
 }
 
-template <int VARIANT, bool PARTIAL, bool POS = false>
-static int launch_ldg(const GbParams& p, const DevProps& dp, cudaStream_t st) {
-  int occ = 0;
-  MB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, gb_accumulate_kernel<VARIANT, PARTIAL, POS>, kGbThreads, 0));
-  const long long nchunks = (p.nrows + 31) / 32;
-  long long grid = (long long)dp.sm_count * (occ < 1 ? 1 : occ);
-  const long long need = (nchunks + kGbWarps - 1) / kGbWarps;
-  if (grid > need) grid = need;
-  gb_accumulate_kernel<VARIANT, PARTIAL, POS><<<(unsigned)grid, kGbThreads, 0, st>>>(p);
-  MB_LAUNCH_CHECK("gb_accumulate_kernel");
-  return 0;
-}
-
-static int gb_launch(mb200_gb_table* t, const long long* keys, const void* const* vals, const void* const* pcnt,
-                     const long long* psize, long long nrows, bool partial, cudaStream_t st) {
-  if (nrows == 0) return 0;
-  DevProps dp;
-  if (int rc = dev_props(&dp)) return rc;
+// kernel parameters of table `t` over `nrows` rows of `keys`; the launchers add the value columns
+static GbParams gb_params(const mb200_gb_table* t, const long long* keys, long long nrows) {
   GbParams p;
   memset(&p, 0, sizeof(p));
   p.slots = t->slots;
@@ -1051,6 +989,105 @@ static int gb_launch(mb200_gb_table* t, const long long* keys, const void* const
   p.kbase = t->kbase;
   p.present = t->present;
   p.keys = keys;
+  p.nrows = nrows;
+  return p;
+}
+
+// MB200_GB_VARIANT=1 sends every row through the direct-load kernel; it is an on / off switch: unset or any other
+// value, full tiles take the TMA-staged kernel wherever it applies.  Read per call so one process can compare the two.
+// Measured on an H100 80GB HBM3 (400 W power limit), 2^27 rows, V = 8, fresh table per pass, uniform keys, ms TMA /
+// direct: G = 65536 dense 5.3 / 6.1, hashed 6.4 / 7.2; G = 1e6 (64 MB dense, 96 MB hashed: both larger than the 50 MB
+// L2) dense 13.6 / 13.4, hashed 21.5 / 21.9.  With skewed keys only the TMA kernel has the hot-group cache (6.1 ms
+// against 81 at G = 1e6).  So the TMA kernel is taken at every size.
+static bool gb_direct_only() {
+  const char* e = getenv("MB200_GB_VARIANT");
+  return e && e[0] == '1';
+}
+
+// MB200_GB_SMEM=0 keeps dense tables out of shared memory, so that small key ranges reach the global-table kernels
+static bool gb_smem_tables() {
+  const char* e = getenv("MB200_GB_SMEM");
+  return !(e && e[0] == '0');
+}
+
+// direct-load kernels (gb_accumulate_kernel, gb_arg_kernel): as many CTAs as fit, but no more than one warp per 32 rows
+template <typename... K, typename... A>
+static int launch_direct(void (*kern)(GbParams, K...), const char* name, const GbParams& p, const DevProps& dp,
+                         cudaStream_t st, A... args) {
+  int occ = 0;
+  MB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kGbThreads, 0));
+  const long long nchunks = (p.nrows + 31) / 32;
+  long long grid = (long long)dp.sm_count * (occ < 1 ? 1 : occ);
+  const long long need = (nchunks + kGbWarps - 1) / kGbWarps;
+  if (grid > need) grid = need;
+  kern<<<(unsigned)grid, kGbThreads, 0, st>>>(p, args...);
+  MB_LAUNCH_CHECK(name);
+  return 0;
+}
+
+// shared-memory table kernels: one CTA per SM, but no more than the rows need
+static unsigned smem_grid(long long nrows, const DevProps& dp) {
+  const long long need = (nrows + kSmemThreads - 1) / kSmemThreads;
+  return (unsigned)(dp.sm_count < need ? dp.sm_count : need);
+}
+
+// Shared-memory layout of table `t` with `nrep` replicas; returns its bytes.
+typedef size_t (*SmemLayoutFn)(const mb200_gb_table* t, int nrep, SmemTableLayout* lay);
+
+// accumulate tables: acc replicas (8 B) | cnt replicas (4 B) | size replicas (4 B) | presence bytes
+static size_t smem_layout_accumulate(const mb200_gb_table* t, int nrep, SmemTableLayout* lay) {
+  const TableArrays ta = table_arrays(t->flags, true);
+  lay->svs = t->vstride + 1;
+  lay->rstride = (int)((((size_t)t->gcap * lay->svs + 15) & ~(size_t)15) + 1);
+  lay->zstride = (int)(t->gcap | 1);
+  lay->nrep = nrep;
+  const size_t elems = (size_t)nrep * lay->rstride;
+  size_t off = 0;
+  lay->acc_off = (unsigned)off;
+  if (ta.acc) off += elems * 8;
+  lay->cnt_off = (unsigned)off;
+  if (ta.cnt) off += (elems * 4 + 15) & ~(size_t)15;
+  lay->size_off = (unsigned)off;
+  if (ta.size) off += (((size_t)nrep * lay->zstride * 4) + 15) & ~(size_t)15;
+  lay->present_off = (unsigned)off;
+  off += ((size_t)t->gcap + 15) & ~(size_t)15;
+  lay->total = (unsigned)off;
+  return off;
+}
+
+// ARG tables: image / position replicas (8 B) | the final images of pass 1 (8 B) | presence bytes
+static size_t smem_layout_arg(const mb200_gb_table* t, int nrep, SmemTableLayout* lay) {
+  memset(lay, 0, sizeof(*lay));
+  lay->svs = t->vstride + 1;
+  const size_t elems1 = (size_t)t->gcap * lay->svs;
+  lay->rstride = (int)(((elems1 + 15) & ~(size_t)15) + 1);
+  lay->nrep = nrep;
+  size_t off = (((size_t)nrep * lay->rstride * 8) + 15) & ~(size_t)15;
+  lay->cnt_off = (unsigned)off;
+  off += elems1 * 8;
+  lay->present_off = (unsigned)off;
+  off += ((size_t)t->gcap + 15) & ~(size_t)15;
+  lay->total = (unsigned)off;
+  return off;
+}
+
+// Bytes of the layout with the most replicas (32, 16, ..., 1) that fits in shared memory; 0 when not even one does.
+// Lanes of a warp that hit the same group then work on different copies: G = 16 runs 2.6x faster with 32 replicas
+// than with one.
+static size_t fit_replicas(SmemLayoutFn layout, const mb200_gb_table* t, const DevProps& dp, SmemTableLayout* lay) {
+  for (int nrep = 32; nrep >= 1; nrep >>= 1) {
+    const size_t bytes = layout(t, nrep, lay);
+    if (bytes <= dp.smem_optin) return bytes;
+  }
+  return 0;
+}
+
+static int gb_launch(mb200_gb_table* t, const long long* keys, const void* const* vals, const void* const* pcnt,
+                     const long long* psize, long long nrows, bool partial, cudaStream_t st) {
+  if (nrows == 0) return 0;
+  DevProps dp;
+  if (int rc = dev_props(&dp)) return rc;
+  GbParams p = gb_params(t, keys, nrows);
   const bool pos = t->flags & (MB200_GB_FIRST | MB200_GB_LAST);
   if (pos && partial) return fail("groupby", "FIRST / LAST tables do not merge partial tables");
   bool aligned = aligned16(keys);
@@ -1065,17 +1102,6 @@ static int gb_launch(mb200_gb_table* t, const long long* keys, const void* const
   if (pos) p.row0 = t->rows;
   else p.psize = psize;
   if (partial && (t->flags & MB200_GB_SIZE) && !psize) return fail("groupby", "null partial size column");
-  p.nrows = nrows;
-  {
-    const char* e = getenv("MB200_GB_POLICY");  // none | last | normal
-    p.policy_mode = (e && e[0] == 'l') ? 1 : ((e && e[0] == 'n' && e[1] == 'o' && e[2] == 'r') ? 2 : ((e && e[0] == 'u') ? 3 : 0));
-    const char* pf = getenv("MB200_GB_PREFETCH");
-    p.prefetch = (pf && pf[0] == '1') ? 1 : 0;
-  }
-  const size_t table_bytes = (size_t)t->cap * sizeof(Slot) + (size_t)t->gcap * t->vstride * 8 *
-                                                                  (((t->flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST)) ? 1 : 0) +
-                                                                   ((t->flags & MB200_GB_COUNT) ? 1 : 0));
-  const int variant = gb_variant_from_env(table_bytes, dp.l2_bytes);
 
   // Pin the accumulator rows (the 2-sector RED target of every row) in the persisting L2 carve-out for the
   // kernels launched below (the carve-out size is the device's cudaDevAttrMaxPersistingL2CacheSize).
@@ -1131,48 +1157,20 @@ static int gb_launch(mb200_gb_table* t, const long long* keys, const void* const
   }
 
   // low-cardinality dense tables: privatise the table in shared memory (MB200_GB_SMEM=0 disables)
-  if (t->dense && !partial) {
-    const char* e = getenv("MB200_GB_SMEM");
-    SmemTableLayout lay;
-    lay.svs = t->vstride + 1;
-    lay.rstride = (int)((((size_t)t->gcap * lay.svs + 15) & ~(size_t)15) + 1);
-    lay.zstride = (int)(t->gcap | 1);
-    size_t off = 0;
-    // as many replicas as fit (conflicting lanes of a warp then work on different copies: G = 16 runs
-    // 2.6x faster with 32 replicas than with one)
-    for (int nrep = 32; nrep >= 1; nrep >>= 1) {
-      const size_t elems = (size_t)nrep * lay.rstride;
-      off = 0;
-      lay.nrep = nrep;
-      lay.acc_off = (unsigned)off;
-      if (t->flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST)) off += elems * 8;
-      lay.cnt_off = (unsigned)off;
-      if (t->flags & MB200_GB_COUNT) off += (elems * 4 + 15) & ~(size_t)15;
-      lay.size_off = (unsigned)off;
-      if (t->flags & MB200_GB_SIZE) off += (((size_t)nrep * lay.zstride * 4) + 15) & ~(size_t)15;
-      lay.present_off = (unsigned)off;
-      off += ((size_t)t->gcap + 15) & ~(size_t)15;
-      lay.total = (unsigned)off;
-      if (off <= dp.smem_optin) break;
-    }
-    if (!(e && e[0] == '0') && off <= dp.smem_optin) {
-      auto kern = pos ? gb_accumulate_smem_kernel<true> : gb_accumulate_smem_kernel<false>;
-      MB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)off));
-      long long grid = dp.sm_count;
-      const long long need = (nrows + kSmemThreads - 1) / kSmemThreads;
-      if (grid > need) grid = need;
-      kern<<<(unsigned)grid, kSmemThreads, off, st>>>(p, lay);
-      MB_LAUNCH_CHECK("gb_accumulate_smem_kernel");
-      return 0;
-    }
+  SmemTableLayout lay;
+  const size_t table_smem = (t->dense && !partial && gb_smem_tables()) ? fit_replicas(smem_layout_accumulate, t, dp, &lay) : 0;
+  if (table_smem) {
+    auto kern = pos ? gb_accumulate_smem_kernel<true> : gb_accumulate_smem_kernel<false>;
+    MB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)table_smem));
+    kern<<<smem_grid(nrows, dp), kSmemThreads, table_smem, st>>>(p, lay);
+    MB_LAUNCH_CHECK("gb_accumulate_smem_kernel");
+    return 0;
   }
-  if (variant == 0 && !partial && aligned && t->nvals <= 8 && nrows >= kTileRows) {
+  if (!gb_direct_only() && !partial && aligned && t->nvals <= 8 && nrows >= kTileRows) {
     const long long ntiles = nrows / kTileRows;
     const bool hot = t->skewed && !(t->flags & (MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST | MB200_GB_SIZE));
-    // hashed tables: a 2-stage ring lets 5 CTAs share an SM instead of 4 (the probe chain wants warps, not staging
-    // depth); MB200_GB_STAGES=3 restores the 3-stage ring for comparison
-    const char* se = getenv("MB200_GB_STAGES");
-    const bool two = !hot && !t->dense && !(se && se[0] == '3');
+    // hashed tables: a 2-stage ring lets 5 CTAs share an SM instead of 4 (the probe chain wants warps, not staging depth)
+    const bool two = !hot && !t->dense;
     const size_t smem = hot   ? (size_t)hot_offset(kHotStages) + ((t->flags & MB200_GB_COUNT) ? kHotBytes : kHotBytesSum)
                         : two ? (size_t)2 * kStageBytes + 2 * 2 * sizeof(uint64_t)
                               : (size_t)kGbStages * kStageBytes + 2 * kGbStages * sizeof(uint64_t);
@@ -1196,14 +1194,10 @@ static int gb_launch(mb200_gb_table* t, const long long* keys, const void* const
     p.row0 += done;
     p.nrows = nrows - done;
   }
-  if (variant == 2) {
-    if (pos) return launch_ldg<1, false, true>(p, dp, st);
-    if (partial) return launch_ldg<1, true>(p, dp, st);
-    return launch_ldg<1, false>(p, dp, st);
-  }
-  if (pos) return launch_ldg<0, false, true>(p, dp, st);
-  if (partial) return launch_ldg<0, true>(p, dp, st);
-  return launch_ldg<0, false>(p, dp, st);
+  auto kern = pos       ? gb_accumulate_kernel<false, true>
+              : partial ? gb_accumulate_kernel<true, false>
+                        : gb_accumulate_kernel<false, false>;
+  return launch_direct(kern, "gb_accumulate_kernel", p, dp, st);
 }
 
 
@@ -1261,7 +1255,7 @@ __global__ void __launch_bounds__(kGbThreads, PASS == 1 ? 4 : 5) gb_arg_kernel(c
       const long long k0 = __shfl_sync(0xffffffffu, k, 0);  // rows past the end join lane 0's peer group
       k = valid ? k : k0;
     }
-    const int gid = resolve_gid(p, k, 0);  // pass 2: every key is in the table already, nothing is inserted
+    const int gid = resolve_gid(p, k);  // pass 2: every key is in the table already, nothing is inserted
     if (PASS == 1 && p.dense && p.nvals == 0 && valid && gid < gcap) dense_mark(p, gid);
     for (int c0 = 0; c0 < p.nvals; c0 += 8) {
       const int nc = (p.nvals - c0) < 8 ? (p.nvals - c0) : 8;
@@ -1406,78 +1400,30 @@ __global__ void __launch_bounds__(kSmemThreads, 1) gb_arg_smem_kernel(const __gr
       if (s_present[g]) reinterpret_cast<unsigned char*>(p.present)[g] = 1;
 }
 
-template <int PASS>
-static int launch_arg_ldg(const GbParams& p, unsigned int i64_mask, const DevProps& dp, cudaStream_t st) {
-  int occ = 0;
-  MB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, gb_arg_kernel<PASS>, kGbThreads, 0));
-  const long long nchunks = (p.nrows + 31) / 32;
-  long long grid = (long long)dp.sm_count * (occ < 1 ? 1 : occ);
-  const long long need = (nchunks + kGbWarps - 1) / kGbWarps;
-  if (grid > need) grid = need;
-  gb_arg_kernel<PASS><<<(unsigned)grid, kGbThreads, 0, st>>>(p, i64_mask);
-  MB_LAUNCH_CHECK("gb_arg_kernel");
-  return 0;
-}
-
 static int gb_arg_launch(mb200_gb_table* t, const long long* keys, const void* const* vals, unsigned int i64_mask,
                          long long nrows, cudaStream_t st) {
   if (nrows == 0) return 0;
   DevProps dp;
   if (int rc = dev_props(&dp)) return rc;
-  GbParams p;
-  memset(&p, 0, sizeof(p));
-  p.slots = t->slots;
-  p.mask = (unsigned int)(t->cap - 1);
-  p.cap = t->cap;
-  p.acc = t->acc;
-  p.cnt = t->cnt;
-  p.gcap = t->gcap;
-  p.nvals = t->nvals;
-  p.vstride = t->vstride;
-  p.flags = t->flags;
-  p.meta = t->meta;
-  p.dense = t->dense;
-  p.kbase = t->kbase;
-  p.present = t->present;
-  p.keys = keys;
-  p.nrows = nrows;
+  GbParams p = gb_params(t, keys, nrows);
   for (int c = 0; c < t->nvals; ++c) {
     p.vals[c] = vals[c];
     if (!p.vals[c]) return fail("mb200_gb_accumulate_arg", "null value column");
   }
-  if (t->dense && !(getenv("MB200_GB_SMEM") && getenv("MB200_GB_SMEM")[0] == '0')) {
-    SmemTableLayout lay;
-    memset(&lay, 0, sizeof(lay));
-    lay.svs = t->vstride + 1;
-    const size_t elems1 = (size_t)t->gcap * lay.svs;
-    lay.rstride = (int)(((elems1 + 15) & ~(size_t)15) + 1);
-    size_t off = 0;
-    for (int nrep = 32; nrep >= 1; nrep >>= 1) {
-      lay.nrep = nrep;
-      lay.acc_off = 0;
-      off = (((size_t)nrep * lay.rstride * 8) + 15) & ~(size_t)15;
-      lay.cnt_off = (unsigned)off;
-      off += elems1 * 8;
-      lay.present_off = (unsigned)off;
-      off += ((size_t)t->gcap + 15) & ~(size_t)15;
-      lay.total = (unsigned)off;
-      if (off <= dp.smem_optin) break;
-    }
-    if (off <= dp.smem_optin) {
-      long long grid = dp.sm_count;
-      const long long need = (nrows + kSmemThreads - 1) / kSmemThreads;
-      if (grid > need) grid = need;
-      MB_CUDA(cudaFuncSetAttribute(gb_arg_smem_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)off));
-      MB_CUDA(cudaFuncSetAttribute(gb_arg_smem_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)off));
-      gb_arg_smem_kernel<1><<<(unsigned)grid, kSmemThreads, off, st>>>(p, lay, i64_mask);
-      MB_LAUNCH_CHECK("gb_arg_smem_kernel");
-      gb_arg_smem_kernel<2><<<(unsigned)grid, kSmemThreads, off, st>>>(p, lay, i64_mask);
-      MB_LAUNCH_CHECK("gb_arg_smem_kernel");
-      return 0;
-    }
+  SmemTableLayout lay;
+  const size_t table_smem = (t->dense && gb_smem_tables()) ? fit_replicas(smem_layout_arg, t, dp, &lay) : 0;
+  if (table_smem) {
+    const unsigned grid = smem_grid(nrows, dp);
+    MB_CUDA(cudaFuncSetAttribute(gb_arg_smem_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)table_smem));
+    MB_CUDA(cudaFuncSetAttribute(gb_arg_smem_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)table_smem));
+    gb_arg_smem_kernel<1><<<grid, kSmemThreads, table_smem, st>>>(p, lay, i64_mask);
+    MB_LAUNCH_CHECK("gb_arg_smem_kernel");
+    gb_arg_smem_kernel<2><<<grid, kSmemThreads, table_smem, st>>>(p, lay, i64_mask);
+    MB_LAUNCH_CHECK("gb_arg_smem_kernel");
+    return 0;
   }
-  if (int rc = launch_arg_ldg<1>(p, i64_mask, dp, st)) return rc;
-  return launch_arg_ldg<2>(p, i64_mask, dp, st);
+  if (int rc = launch_direct(gb_arg_kernel<1>, "gb_arg_kernel", p, dp, st, i64_mask)) return rc;
+  return launch_direct(gb_arg_kernel<2>, "gb_arg_kernel", p, dp, st, i64_mask);
 }
 
 }  // namespace mb200
@@ -1499,22 +1445,31 @@ extern "C" int mb200_gb_create(mb200_gb_table** table, int64_t group_capacity, i
   return gb_create_impl(table, group_capacity, nvals, flags, false, 0, DenseArrays{}, stream);
 }
 
+// Arguments of a dense table over [key_min, key_max]: a range of at most 2^29 keys (left in *range) and, when the
+// caller owns the arrays (`borrowed`), the presence array and every other array the flags need, all 16-byte aligned.
+// Arrays given without the presence array are refused.
+static int check_dense_args(const char* fn, int64_t key_min, int64_t key_max, int flags, const DenseArrays& ext,
+                            bool borrowed, int64_t* range) {
+  if (key_max < key_min) return fail(fn, "empty key range");
+  const unsigned long long r = (unsigned long long)key_max - (unsigned long long)key_min + 1ULL;
+  if (r == 0 || r > (1ULL << 29)) return fail(fn, "key range above 2^29");
+  *range = (int64_t)r;
+  if (!borrowed) return (ext.acc || ext.cnt || ext.size) ? fail(fn, "caller-owned arrays need the presence array too") : 0;
+  const TableArrays ta = table_arrays(flags, true);
+  if (!ext.present || (ta.acc && !ext.acc) || (ta.cnt && !ext.cnt) || (ta.size && !ext.size))
+    return fail(fn, "caller-owned arrays: every array the flags need must be given");
+  if (!aligned16(ext.acc) || !aligned16(ext.cnt) || !aligned16(ext.size) || !aligned16(ext.present))
+    return fail(fn, "caller-owned arrays must be 16-byte aligned");
+  return 0;
+}
+
 extern "C" int mb200_gb_create_dense(mb200_gb_table** table, int64_t key_min, int64_t key_max, int nvals, int flags,
                                      void* acc, void* cnt, void* size, void* present, mb200_stream_t stream) {
-  if (key_max < key_min) return fail("mb200_gb_create_dense", "empty key range");
-  const unsigned long long range = (unsigned long long)key_max - (unsigned long long)key_min + 1ULL;
-  if (range == 0 || range > (1ULL << 29)) return fail("mb200_gb_create_dense", "key range above 2^29");
-  DenseArrays ext{acc, cnt, size, present};
-  if (present) {
-    const bool need_acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST | kGbArg);
-    if ((need_acc && !acc) || ((flags & (MB200_GB_COUNT | kGbArg)) && !cnt) || ((flags & MB200_GB_SIZE) && !size))
-      return fail("mb200_gb_create_dense", "caller-owned arrays: every array the flags need must be given");
-    if (!aligned16(acc) || !aligned16(cnt) || !aligned16(size) || !aligned16(present))
-      return fail("mb200_gb_create_dense", "caller-owned arrays must be 16-byte aligned");
-  } else if (acc || cnt || size) {
-    return fail("mb200_gb_create_dense", "caller-owned arrays need the presence array too");
-  }
-  return gb_create_impl(table, (int64_t)range, nvals, flags, true, key_min, ext, stream);
+  const DenseArrays ext{acc, cnt, size, present};
+  int64_t range;
+  if (int rc = check_dense_args("mb200_gb_create_dense", key_min, key_max, flags, ext, present != nullptr, &range))
+    return rc;
+  return gb_create_impl(table, range, nvals, flags, true, key_min, ext, stream);
 }
 
 namespace mb200 {
@@ -1526,16 +1481,10 @@ __global__ void gb_inherit_overflow_kernel(GbMeta* child, const GbMeta* parent) 
 extern "C" int mb200_gb_adopt_dense(mb200_gb_table** table, int64_t key_min, int64_t key_max, int nvals, int flags,
                                     void* acc, void* cnt, void* size, void* present, const mb200_gb_table* parent,
                                     mb200_stream_t stream) {
-  if (key_max < key_min) return fail("mb200_gb_adopt_dense", "empty key range");
-  const unsigned long long range = (unsigned long long)key_max - (unsigned long long)key_min + 1ULL;
-  if (range == 0 || range > (1ULL << 29)) return fail("mb200_gb_adopt_dense", "key range above 2^29");
-  const bool need_acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST | kGbArg);
-  if (!present || (need_acc && !acc) || ((flags & (MB200_GB_COUNT | kGbArg)) && !cnt) || ((flags & MB200_GB_SIZE) && !size))
-    return fail("mb200_gb_adopt_dense", "every array the flags need must be given");
-  if (!aligned16(acc) || !aligned16(cnt) || !aligned16(size) || !aligned16(present))
-    return fail("mb200_gb_adopt_dense", "arrays must be 16-byte aligned");
-  DenseArrays ext{acc, cnt, size, present};
-  if (int rc = gb_create_impl(table, (int64_t)range, nvals, flags, true, key_min, ext, stream, /*init_arrays=*/false))
+  const DenseArrays ext{acc, cnt, size, present};
+  int64_t range;
+  if (int rc = check_dense_args("mb200_gb_adopt_dense", key_min, key_max, flags, ext, true, &range)) return rc;
+  if (int rc = gb_create_impl(table, range, nvals, flags, true, key_min, ext, stream, /*init_arrays=*/false))
     return rc;
   if (parent) {
     gb_inherit_overflow_kernel<<<1, 1, 0, (cudaStream_t)stream>>>((*table)->meta, parent->meta);
@@ -1610,6 +1559,18 @@ static int gb_create_impl(mb200_gb_table** table, int64_t group_capacity, int nv
   t->flags = flags;
   cudaError_t e;
   const size_t accb = (size_t)t->gcap * t->vstride * 8;
+  const TableArrays ta = table_arrays(flags, dense);
+  // allocates a dense array the caller does not own, then sets every word to `init`: a memset for 0, the fill kernel
+  // for anything else (INT64_MAX = bytes ff..ff 7f is not a byte pattern)
+  auto init_array = [&](void** arr, size_t bytes, long long init) -> cudaError_t {
+    if (dense && !t->borrowed)
+      if (cudaError_t err = cudaMallocAsync(arr, bytes, st)) return err;
+    if (init == 0) return cudaMemsetAsync(*arr, 0, bytes, st);
+    gb_fill_kernel<<<(unsigned)dp.sm_count * 4, 256, 0, st>>>(static_cast<long long*>(*arr), (long long)(bytes / 8), init);
+    const cudaError_t err = cudaGetLastError();
+    if (err == cudaSuccess) g_launches.fetch_add(1);
+    return err;
+  };
 #define MB_TRY(call)                \
   do {                              \
     e = (call);                     \
@@ -1628,62 +1589,28 @@ static int gb_create_impl(mb200_gb_table** table, int64_t group_capacity, int nv
   } else {
     const size_t slot_b = ((size_t)t->cap * sizeof(Slot) + 255) & ~(size_t)255;
     const size_t acc_b = (accb + 255) & ~(size_t)255;
-    const bool has_acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST | kGbArg);
     const size_t size_b = (((size_t)t->gcap * 8) + 255) & ~(size_t)255;
-    t->arena_bytes = slot_b + (has_acc ? acc_b : 0) + ((flags & (MB200_GB_COUNT | kGbArg)) ? acc_b : 0) +
-                     ((flags & MB200_GB_SIZE) ? size_b : 0);
+    t->arena_bytes = slot_b + (ta.acc ? acc_b : 0) + (ta.cnt ? acc_b : 0) + (ta.size ? size_b : 0);
     MB_TRY(cudaMallocAsync(&t->arena, t->arena_bytes, st));
     char* a = static_cast<char*>(t->arena);
     t->slots = reinterpret_cast<Slot*>(a);
     a += slot_b;
-    if (has_acc) {
+    if (ta.acc) {
       t->acc = reinterpret_cast<double*>(a);
       a += acc_b;
     }
-    if (flags & (MB200_GB_COUNT | kGbArg)) {  // ARGMIN / ARGMAX: the extreme images
+    if (ta.cnt) {
       t->cnt = reinterpret_cast<long long*>(a);
       a += acc_b;
     }
-    if (flags & MB200_GB_SIZE) t->size = reinterpret_cast<long long*>(a);
+    if (ta.size) t->size = reinterpret_cast<long long*>(a);
   }
   MB_TRY(cudaMallocAsync((void**)&t->meta, sizeof(GbMeta), st));
-  if (!init_arrays) {
-    // adopted arrays (mb200_gb_adopt_dense): already hold a merged table, nothing to initialise
-  } else if (flags & MB200_GB_SUM) {
-    if (!t->borrowed && dense) MB_TRY(cudaMallocAsync((void**)&t->acc, accb, st));
-    if (dense) {  // -0.0: the one value no sum can end on (x + -0.0 = x, and sums start from +0.0 in the emit)
-      gb_fill_kernel<<<(unsigned)dp.sm_count * 4, 256, 0, st>>>(reinterpret_cast<long long*>(t->acc),
-                                                               (long long)(accb / 8), (long long)0x8000000000000000ULL);
-      MB_TRY(cudaGetLastError());
-      g_launches.fetch_add(1);
-    } else {
-      MB_TRY(cudaMemsetAsync(t->acc, 0, accb, st));
-    }
-  } else if (flags & (MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST | kGbArg)) {
-    if (!t->borrowed && dense) MB_TRY(cudaMallocAsync((void**)&t->acc, accb, st));
-    // "no value yet": INT64_MAX = bytes ff..ff 7f for min is not a byte pattern; use the fill kernel
-    gb_fill_kernel<<<(unsigned)dp.sm_count * 4, 256, 0, st>>>(reinterpret_cast<long long*>(t->acc),
-                                                             (long long)(accb / 8),
-                                                             (flags & (MB200_GB_MIN | MB200_GB_FIRST | kGbArg))
-                                                                 ? 0x7fffffffffffffffLL
-                                                                 : (long long)0x8000000000000000ULL);
-    MB_TRY(cudaGetLastError());
-    g_launches.fetch_add(1);
-  }
-  if ((flags & kGbArg) && init_arrays) {  // extreme images start below / above every image
-    if (!t->borrowed && dense) MB_TRY(cudaMallocAsync((void**)&t->cnt, accb, st));
-    gb_fill_kernel<<<(unsigned)dp.sm_count * 4, 256, 0, st>>>(
-        t->cnt, (long long)(accb / 8), (flags & MB200_GB_ARGMAX) ? (long long)0x8000000000000000ULL : 0x7fffffffffffffffLL);
-    MB_TRY(cudaGetLastError());
-    g_launches.fetch_add(1);
-  }
-  if ((flags & MB200_GB_COUNT) && init_arrays) {
-    if (!t->borrowed && dense) MB_TRY(cudaMallocAsync((void**)&t->cnt, accb, st));
-    MB_TRY(cudaMemsetAsync(t->cnt, 0, accb, st));
-  }
-  if ((flags & MB200_GB_SIZE) && init_arrays) {
-    if (!t->borrowed && dense) MB_TRY(cudaMallocAsync((void**)&t->size, (size_t)t->gcap * 8, st));
-    MB_TRY(cudaMemsetAsync(t->size, 0, (size_t)t->gcap * 8, st));
+  // adopted arrays (mb200_gb_adopt_dense) already hold a merged table: nothing to initialise
+  if (init_arrays) {
+    if (ta.acc) MB_TRY(init_array((void**)&t->acc, accb, ta.acc_init));
+    if (ta.cnt) MB_TRY(init_array((void**)&t->cnt, accb, ta.cnt_init));
+    if (ta.size) MB_TRY(init_array((void**)&t->size, (size_t)t->gcap * 8, 0));
   }
 #undef MB_TRY
   gb_init_kernel<<<(unsigned)(dense ? 1 : (t->cap + 255) / 256), 256, 0, st>>>(t->slots, t->cap, t->meta);
@@ -1765,14 +1692,11 @@ extern "C" int mb200_gb_accumulate_arg(mb200_gb_table* t, const int64_t* keys, c
 static int dense_finalize_presence(mb200_gb_table* t, cudaStream_t st) {
   const long long n = t->win_hi - t->win_lo;
   if (n <= 0) return 0;
-  const long long init = (t->flags & MB200_GB_SUM)   ? (long long)0x8000000000000000ULL
-                         : (t->flags & (MB200_GB_MIN | MB200_GB_FIRST | kGbArg)) ? 0x7fffffffffffffffLL
-                                                     : (long long)0x8000000000000000ULL;
   // ARGMIN / ARGMAX: cnt holds images, not counts; presence is a moved position or a marked byte
   dense_presence_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
       reinterpret_cast<unsigned char*>(t->present), reinterpret_cast<const long long*>(t->acc),
       (t->flags & kGbArg) ? nullptr : t->cnt, t->size,
-      t->win_lo, t->win_hi, t->nvals, t->vstride, init);
+      t->win_lo, t->win_hi, t->nvals, t->vstride, table_arrays(t->flags, true).acc_init);
   MB_LAUNCH_CHECK("dense_presence_kernel");
   return 0;
 }
