@@ -39,9 +39,9 @@ extern "C" {
 
 /* 2: round 2 (key statistics, async dense emit, expand / concat / comm entry points); 3: + the Fold template's
  * cumulative scans (mb200_cum_*); 4: + MB200_GB_FIRST / MB200_GB_LAST group tables (row positions, NULL value
- * columns); 5: + MB200_GB_ARGMIN / MB200_GB_ARGMAX group tables and mb200_gb_accumulate_arg.  Checked by the binding
- * at load time (modin_b200/_lib.py). */
-#define MB200_ABI_VERSION 5
+ * columns); 5: + MB200_GB_ARGMIN / MB200_GB_ARGMAX group tables and mb200_gb_accumulate_arg; 6: + MB200_GB_VAR group
+ * tables and mb200_gb_accumulate_m2.  Checked by the binding at load time (modin_b200/_lib.py). */
+#define MB200_ABI_VERSION 6
 #define MB200_MAX_COLS 32 /* max columns per launch == Modin's MinColumnPartitionSize (envvars.py:1149-1190) */
 
 typedef void* mb200_stream_t;
@@ -140,7 +140,12 @@ enum mb200_gb_flags {
   /* the first row holding the group's extreme value; each excludes every other flag (see mb200_gb_accumulate_arg):
    * cnt[g][v] = min / max of the value's order-preserving int64 image, acc[g][v] = min(position) of the rows holding it */
   MB200_GB_ARGMIN = 128,
-  MB200_GB_ARGMAX = 256
+  MB200_GB_ARGMAX = 256,
+  /* groupby.var / std: a VAR table is exactly SUM | COUNT | VAR.  It has one more float64 array, m2[g][v], which the
+   * library allocates for dense tables too (it is not among the caller-owned arrays of mb200_gb_create_dense) and
+   * which starts at 0.  Pass 1 fills acc / cnt (mb200_gb_accumulate, mb200_gb_merge_partial); pass 2 fills m2
+   * (mb200_gb_accumulate_m2) */
+  MB200_GB_VAR = 512
 };
 
 /* ======================= runtime / memory ================================== */
@@ -281,6 +286,16 @@ int mb200_gb_merge_partial(mb200_gb_table* table, const int64_t* keys,
  * order of the atomics.  Called once per table: a second call is refused (positions would not run on). */
 int mb200_gb_accumulate_arg(mb200_gb_table* table, const int64_t* keys, const void* const* vals, uint32_t i64_mask,
                             int64_t nrows, mb200_stream_t stream);
+/* Pass 2 of a VAR table (groupby.var / std): m2[g][v] += the squared deviations of the inputs from the group's mean
+ * m = acc[g][v] / cnt[g][v], as pass 1 left it.  Raw form (cnts == NULL): vals[nvals][nrows] float64 values, each
+ * non-NaN x adds (x - m)^2.  Partial form: the rows of other VAR tables' emits, vals = their sums S_p, cnts = their
+ * counts n_p (int64), m2s = their M2_p; each row with n_p > 0 adds M2_p + n_p (S_p / n_p - m)^2 (Chan et al.'s
+ * pairwise update).  Keys that are not in the table, and (group, column) pairs that pass 1 gave no value, add nothing.
+ * May be called any number of times, in either form; after the first call mb200_gb_accumulate and
+ * mb200_gb_merge_partial refuse the table (its means must not move).  Float atomics: the summation order is
+ * run-dependent, the result is within the bound stated in README.md, not bit for bit. */
+int mb200_gb_accumulate_m2(mb200_gb_table* table, const int64_t* keys, const void* const* vals,
+                           const void* const* cnts, const void* const* m2s, int64_t nrows, mb200_stream_t stream);
 /* Synchronises `stream`; returns number of groups and whether capacity was exceeded. */
 int mb200_gb_ngroups(mb200_gb_table* table, int64_t* ngroups, int* overflow,
                      mb200_stream_t stream);
@@ -289,7 +304,8 @@ size_t mb200_gb_emit_scratch_bytes(int64_t ngroups);
 /* Write the result block: out_keys[ngroups] (ascending iff sort), out_sums[nvals][ngroups],
  * out_cnts[nvals][ngroups] (int64, may be NULL), out_sizes[ngroups] (may be NULL).
  * FIRST / LAST and ARGMIN / ARGMAX tables write int64 positions into out_sums, -1 where the group has no non-NaN
- * value in the column (mb200_take turns -1 into NaN). */
+ * value in the column (mb200_take turns -1 into NaN).  A VAR table's out_sums holds 2 * nvals pointers: the sums
+ * out_sums[0 .. nvals), then the M2s out_sums[nvals .. 2 nvals) (float64; an entry may be NULL). */
 int mb200_gb_emit(mb200_gb_table* table, int64_t ngroups, int sort, int64_t* out_keys,
                   void* const* out_sums, void* const* out_cnts, int64_t* out_sizes,
                   void* scratch, mb200_stream_t stream);

@@ -87,6 +87,8 @@ struct mb200_gb_table {
   size_t arena_bytes;
   long long rows;  // rows accumulated so far: the position of the next accumulate call's first row (FIRST / LAST)
   int arg_filled;  // ARGMIN / ARGMAX: mb200_gb_accumulate_arg has run (it runs once per table)
+  double* m2;      // VAR: sums of squared deviations [gcap][vstride], always the library's (in the arena when hashed)
+  int m2_filled;   // VAR: mb200_gb_accumulate_m2 has run, so the means are final and pass-1 calls are refused
 };
 
 namespace mb200 {
@@ -94,6 +96,7 @@ namespace mb200 {
 constexpr int kGbThreads = 256;
 constexpr int kGbWarps = kGbThreads / 32;
 constexpr int kGbArg = MB200_GB_ARGMIN | MB200_GB_ARGMAX;  // groupby.idxmin / idxmax tables
+constexpr int kGbVarTable = MB200_GB_SUM | MB200_GB_COUNT | MB200_GB_VAR;  // groupby.var / std: the only VAR combination
 constexpr int kColStride = 34;  // doubles; 34 = 2 (mod 16) -> conflict-free transposed reads
 // TMA-staged kernel
 constexpr int kTileRows = 256;
@@ -769,6 +772,8 @@ struct EmitParams {
   void* out_sums[MB200_MAX_COLS];
   void* out_cnts[MB200_MAX_COLS];
   long long* out_sizes;
+  const double* m2;  // VAR tables
+  void* out_m2[MB200_MAX_COLS];
 };
 
 __global__ void gb_emit_kernel(const __grid_constant__ EmitParams p) {
@@ -796,6 +801,7 @@ __global__ void gb_emit_kernel(const __grid_constant__ EmitParams p) {
       static_cast<double*>(p.out_sums[v])[i] = val;
     }
     if (p.out_cnts[v] && p.cnt) static_cast<long long*>(p.out_cnts[v])[i] = p.cnt[(size_t)g * p.vstride + v];
+    if (p.out_m2[v] && p.m2) static_cast<double*>(p.out_m2[v])[i] = p.m2[(size_t)g * p.vstride + v];
   }
 }
 
@@ -955,8 +961,9 @@ static long long next_pow2(long long v) {
 //        LAST from INT64_MIN.
 //   cnt: non-NaN counts from 0, or an ARG table's extreme images: from INT64_MIN for ARGMAX, INT64_MAX for ARGMIN.
 //   size: rows per group, from 0.
+//   m2: VAR tables' sums of squared deviations from the group means, float64 from 0.
 struct TableArrays {
-  bool acc, cnt, size;
+  bool acc, cnt, size, m2;
   long long acc_init, cnt_init;
 };
 static TableArrays table_arrays(int flags, bool dense) {
@@ -965,6 +972,7 @@ static TableArrays table_arrays(int flags, bool dense) {
   a.acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST | kGbArg);
   a.cnt = flags & (MB200_GB_COUNT | kGbArg);
   a.size = flags & MB200_GB_SIZE;
+  a.m2 = flags & MB200_GB_VAR;
   a.acc_init = (flags & MB200_GB_SUM) ? (dense ? lo : 0) : (flags & (MB200_GB_MIN | MB200_GB_FIRST | kGbArg)) ? hi : lo;
   a.cnt_init = (flags & MB200_GB_ARGMAX) ? lo : (flags & MB200_GB_ARGMIN) ? hi : 0;
   return a;
@@ -1426,6 +1434,213 @@ static int gb_arg_launch(mb200_gb_table* t, const long long* keys, const void* c
   return launch_direct(gb_arg_kernel<2>, "gb_arg_kernel", p, dp, st, i64_mask);
 }
 
+// ---------------------------------------------------------------- VAR tables (groupby.var / std): the centred pass
+// Pass 1 is the SUM | COUNT accumulate (mb200_gb_accumulate / mb200_gb_merge_partial, kernels unchanged: they never read
+// the VAR bit).  Pass 2 (mb200_gb_accumulate_m2) adds, per (group, column), the squared deviations from the group's
+// mean m = acc / cnt into m2: (x - m)^2 for a raw value, M2_p + n_p (S_p / n_p - m)^2 for the row (S_p, n_p, M2_p) of
+// another table's emit.  A (group, column) without a pass-1 value (cnt = 0) has no mean, and its values are skipped.
+struct VarParams {
+  double* m2;
+  const void* pm2[MB200_MAX_COLS];  // partial M2 columns (PARTIAL only)
+};
+
+// Group id of every lane's key, or gcap when the key is not in the table: the probe of resolve_gid without the insert
+// (pass 2 adds no group) and without the overflow flag (a key outside a dense range is simply not in the table).
+__device__ __forceinline__ int lookup_gid(const GbParams& p, long long k) {
+  if (p.dense) {
+    const unsigned long long d = (unsigned long long)k - (unsigned long long)p.kbase;
+    return d >= (unsigned long long)p.gcap ? (int)p.gcap : (int)d;
+  }
+  const int lane = threadIdx.x & 31;
+  const unsigned int peers = __match_any_sync(0xffffffffu, (unsigned long long)k);
+  const int leader = __ffs(peers) - 1;
+  unsigned int bucket = hash_key(k) & (p.mask >> 1);
+  const int gid = __shfl_sync(0xffffffffu, probe_find(p, k, lane == leader, bucket), leader);
+  return gid < 0 ? (int)p.gcap : gid;
+}
+
+
+// direct loads, dense or hashed tables: the mapping of gb_arg_kernel (warp = 32 rows, value tile transposed through
+// shared memory, 8 lanes on the 8 columns of one group's 64-byte row of acc / cnt / m2)
+// (4 CTAs per SM: at 5 the 48-register budget spills, as ARG pass 1 does)
+template <bool PARTIAL>
+__global__ void __launch_bounds__(kGbThreads, 4) gb_var_kernel(const __grid_constant__ GbParams p,
+                                                               const __grid_constant__ VarParams v) {
+  __shared__ double s_tile[kGbWarps][8 * kColStride];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long nchunks = (p.nrows + 31) >> 5;
+  const long long wstride = (long long)gridDim.x * kGbWarps;
+  const int gcap = (int)p.gcap;
+  const uint64_t pol = l2_policy_evict_first();
+  for (long long ch = (long long)blockIdx.x * kGbWarps + warp; ch < nchunks; ch += wstride) {
+    const long long base = ch << 5;
+    const long long row = base + lane;
+    const bool valid = row < p.nrows;
+    long long k = valid ? ldg_stream_i64(p.keys + row, pol) : 0;
+    double x[8];
+    {
+      const int nc = p.nvals < 8 ? p.nvals : 8;
+#pragma unroll
+      for (int c = 0; c < 8; ++c)
+        x[c] = (c < nc && valid) ? ldg_stream_f64(static_cast<const double*>(p.vals[c]) + row, pol) : 0.0;
+    }
+    {
+      const long long k0 = __shfl_sync(0xffffffffu, k, 0);  // rows past the end join lane 0's peer group
+      k = valid ? k : k0;
+    }
+    const int gid = lookup_gid(p, k);
+    for (int c0 = 0; c0 < p.nvals; c0 += 8) {
+      const int nc = (p.nvals - c0) < 8 ? (p.nvals - c0) : 8;
+      if (c0 > 0) {
+#pragma unroll
+        for (int c = 0; c < 8; ++c)
+          x[c] = (c < nc && valid) ? ldg_stream_f64(static_cast<const double*>(p.vals[c0 + c]) + row, pol) : 0.0;
+      }
+      double* tile = s_tile[warp];
+#pragma unroll
+      for (int c = 0; c < 8; ++c) tile[c * kColStride + lane] = x[c];
+      __syncwarp();
+      const int c = lane & 7;
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        const int r = 4 * kk + (lane >> 3);
+        const int g = __shfl_sync(0xffffffffu, gid, r);
+        const double xv = tile[c * kColStride + r];
+        if (base + r < p.nrows && g < gcap && c < nc) {
+          // a raw value x adds (x - m)^2; a partial row (S_p = x, n_p, M2_p) adds M2_p + n_p (S_p / n_p - m)^2.  NaN
+          // values and partial rows with n_p = 0 add nothing.
+          const size_t o = (size_t)g * p.vstride + c0 + c;
+          const long long np = PARTIAL ? static_cast<const long long*>(p.pcnt[c0 + c])[base + r] : 1;
+          const long long n = (PARTIAL ? np != 0 : xv == xv) ? __ldg(p.cnt + o) : 0;
+          if (n > 0) {
+            const double mean = __ldg(p.acc + o) / (double)n;
+            if (PARTIAL) {
+              const double a = xv / (double)np - mean;
+              red_add_f64(v.m2 + o, static_cast<const double*>(v.pm2[c0 + c])[base + r] + (double)np * (a * a));
+            } else {
+              const double d = xv - mean;
+              red_add_f64(v.m2 + o, d * d);
+            }
+          }
+        }
+      }
+      __syncwarp();
+    }
+  }
+}
+
+// low-cardinality dense tables (the ranges gb_accumulate_smem_kernel serves), raw rows: each CTA loads the range's means
+// (and whether each has a pass-1 value) into shared memory once, adds (x - m)^2 into `nrep` replicas of m2 (lane l of a
+// warp on replica l & (nrep - 1)) and folds them into the global m2 once.
+// Layout: acc_off = m2 replicas (8 B), cnt_off = the means (8 B), present_off = one "has a mean" byte per entry.
+__global__ void __launch_bounds__(kSmemThreads, 1) gb_var_smem_kernel(const __grid_constant__ GbParams p,
+                                                                      const SmemTableLayout lay, double* m2) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  double* s_rep = reinterpret_cast<double*>(smem_raw + lay.acc_off);
+  double* s_mean = reinterpret_cast<double*>(smem_raw + lay.cnt_off);
+  unsigned char* s_has = smem_raw + lay.present_off;
+  const int tid = threadIdx.x;
+  const int nv = p.nvals, vs = p.vstride, svs = lay.svs;
+  const int R = (int)p.gcap;
+  const int nrep = lay.nrep, rstride = lay.rstride;
+  for (int i = tid; i < nrep * rstride; i += kSmemThreads) s_rep[i] = 0.0;
+  for (int i = tid; i < R * vs; i += kSmemThreads) {
+    const int g = i / vs, cc = i - g * vs;
+    if (cc >= nv) continue;
+    const long long n = p.cnt[i];
+    s_mean[g * svs + cc] = n > 0 ? p.acc[i] / (double)n : 0.0;
+    s_has[g * svs + cc] = n > 0;
+  }
+  __syncthreads();
+  const uint64_t pol = l2_policy_evict_first();
+  const int rbase = (tid & (nrep - 1)) * rstride;
+  const long long stride = (long long)gridDim.x * kSmemThreads;
+  for (long long row = (long long)blockIdx.x * kSmemThreads + tid; row < p.nrows; row += stride) {
+    const long long key = ldg_stream_i64(p.keys + row, pol);
+    double x[8];
+    {
+      const int nc = nv < 8 ? nv : 8;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) x[c] = (c < nc) ? ldg_stream_f64(static_cast<const double*>(p.vals[c]) + row, pol) : 0.0;
+    }
+    const unsigned long long d = (unsigned long long)key - (unsigned long long)p.kbase;
+    if (d >= (unsigned long long)R) continue;  // not in the table
+    const int gid = (int)d;
+    for (int c0 = 0; c0 < nv; c0 += 8) {
+      const int nc = (nv - c0) < 8 ? (nv - c0) : 8;
+      if (c0 > 0) {
+#pragma unroll
+        for (int c = 0; c < 8; ++c)
+          x[c] = (c < nc) ? ldg_stream_f64(static_cast<const double*>(p.vals[c0 + c]) + row, pol) : 0.0;
+      }
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        const int o = gid * svs + c0 + c;
+        if (c < nc && x[c] == x[c] && s_has[o]) {
+          const double dv = x[c] - s_mean[o];
+          atomicAdd(&s_rep[rbase + o], dv * dv);
+        }
+      }
+    }
+  }
+  __syncthreads();
+  for (int i = tid; i < R * vs; i += kSmemThreads) {
+    const int g = i / vs, cc = i - g * vs;
+    if (cc >= nv) continue;
+    const int o = g * svs + cc;
+    double a = s_rep[o];
+    for (int r = 1; r < nrep; ++r) a += s_rep[r * rstride + o];
+    if (a != 0.0) red_add_f64(m2 + i, a);  // NaN != 0.0: a NaN term reaches the table
+  }
+}
+
+// VAR tables: m2 replicas (8 B) | the means (8 B) | one "has a mean" byte per (group, column)
+static size_t smem_layout_var(const mb200_gb_table* t, int nrep, SmemTableLayout* lay) {
+  memset(lay, 0, sizeof(*lay));
+  lay->svs = t->vstride + 1;
+  const size_t elems1 = (size_t)t->gcap * lay->svs;
+  lay->rstride = (int)(((elems1 + 15) & ~(size_t)15) + 1);
+  lay->nrep = nrep;
+  size_t off = (((size_t)nrep * lay->rstride * 8) + 15) & ~(size_t)15;
+  lay->cnt_off = (unsigned)off;
+  off += elems1 * 8;
+  lay->present_off = (unsigned)off;
+  off += (elems1 + 15) & ~(size_t)15;
+  lay->total = (unsigned)off;
+  return off;
+}
+
+static int gb_var_launch(mb200_gb_table* t, const long long* keys, const void* const* vals, const void* const* cnts,
+                         const void* const* m2s, long long nrows, cudaStream_t st) {
+  if (nrows == 0) return 0;
+  DevProps dp;
+  if (int rc = dev_props(&dp)) return rc;
+  const bool partial = cnts != nullptr;
+  GbParams p = gb_params(t, keys, nrows);
+  VarParams v;
+  memset(&v, 0, sizeof(v));
+  v.m2 = t->m2;
+  for (int c = 0; c < t->nvals; ++c) {
+    p.vals[c] = vals[c];
+    if (!p.vals[c]) return fail("mb200_gb_accumulate_m2", "null value column");
+    if (partial) {
+      p.pcnt[c] = cnts[c];
+      v.pm2[c] = m2s[c];
+      if (!p.pcnt[c] || !v.pm2[c]) return fail("mb200_gb_accumulate_m2", "null partial count or M2 column");
+    }
+  }
+  SmemTableLayout lay;
+  const size_t table_smem = (t->dense && !partial && gb_smem_tables()) ? fit_replicas(smem_layout_var, t, dp, &lay) : 0;
+  if (table_smem) {
+    MB_CUDA(cudaFuncSetAttribute(gb_var_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)table_smem));
+    gb_var_smem_kernel<<<smem_grid(nrows, dp), kSmemThreads, table_smem, st>>>(p, lay, t->m2);
+    MB_LAUNCH_CHECK("gb_var_smem_kernel");
+    return 0;
+  }
+  return partial ? launch_direct(gb_var_kernel<true>, "gb_var_kernel", p, dp, st, v)
+                 : launch_direct(gb_var_kernel<false>, "gb_var_kernel", p, dp, st, v);
+}
+
 }  // namespace mb200
 
 using namespace mb200;
@@ -1540,6 +1755,7 @@ static int gb_create_impl(mb200_gb_table** table, int64_t group_capacity, int nv
     return fail("mb200_gb_create", "FIRST / LAST exclude every other accumulator flag");
   if ((flags & kGbArg) && flags != MB200_GB_ARGMIN && flags != MB200_GB_ARGMAX)
     return fail("mb200_gb_create", "ARGMIN / ARGMAX exclude every other flag");
+  if ((flags & MB200_GB_VAR) && flags != kGbVarTable) return fail("mb200_gb_create", "a VAR table is SUM | COUNT | VAR");
   DevProps dp;
   if (int rc = dev_props(&dp)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
@@ -1590,7 +1806,7 @@ static int gb_create_impl(mb200_gb_table** table, int64_t group_capacity, int nv
     const size_t slot_b = ((size_t)t->cap * sizeof(Slot) + 255) & ~(size_t)255;
     const size_t acc_b = (accb + 255) & ~(size_t)255;
     const size_t size_b = (((size_t)t->gcap * 8) + 255) & ~(size_t)255;
-    t->arena_bytes = slot_b + (ta.acc ? acc_b : 0) + (ta.cnt ? acc_b : 0) + (ta.size ? size_b : 0);
+    t->arena_bytes = slot_b + (ta.acc ? acc_b : 0) + (ta.cnt ? acc_b : 0) + (ta.m2 ? acc_b : 0) + (ta.size ? size_b : 0);
     MB_TRY(cudaMallocAsync(&t->arena, t->arena_bytes, st));
     char* a = static_cast<char*>(t->arena);
     t->slots = reinterpret_cast<Slot*>(a);
@@ -1603,9 +1819,19 @@ static int gb_create_impl(mb200_gb_table** table, int64_t group_capacity, int nv
       t->cnt = reinterpret_cast<long long*>(a);
       a += acc_b;
     }
+    if (ta.m2) {
+      t->m2 = reinterpret_cast<double*>(a);
+      a += acc_b;
+    }
     if (ta.size) t->size = reinterpret_cast<long long*>(a);
   }
   MB_TRY(cudaMallocAsync((void**)&t->meta, sizeof(GbMeta), st));
+  // m2 is never the caller's (so the dense create / adopt signatures need no m2 argument) and starts at 0 even in an
+  // adopted table: the element-wise merge of dense tables across GPUs cannot merge sums of squared deviations
+  if (ta.m2) {
+    if (dense) MB_TRY(cudaMallocAsync((void**)&t->m2, accb, st));
+    MB_TRY(cudaMemsetAsync(t->m2, 0, accb, st));
+  }
   // adopted arrays (mb200_gb_adopt_dense) already hold a merged table: nothing to initialise
   if (init_arrays) {
     if (ta.acc) MB_TRY(init_array((void**)&t->acc, accb, ta.acc_init));
@@ -1635,6 +1861,7 @@ extern "C" int mb200_gb_destroy(mb200_gb_table* t, mb200_stream_t stream) {
     if (t->size) cudaFreeAsync(t->size, st);
     if (t->present) cudaFreeAsync(t->present, st);
   }
+  if (t->m2 && !t->arena) cudaFreeAsync(t->m2, st);
   if (t->blockoff) cudaFreeAsync(t->blockoff, st);
   if (t->persisted) l2_carveout_release();  // the last table hands the carve-out back to normally managed L2
   delete t;
@@ -1656,6 +1883,7 @@ extern "C" int mb200_gb_accumulate(mb200_gb_table* t, const int64_t* keys, const
   if (nrows < 0) return fail("mb200_gb_accumulate", "negative nrows");
   if (nrows > 0 && !keys) return fail("mb200_gb_accumulate", "null keys");
   if (t->flags & kGbArg) return fail("mb200_gb_accumulate", "ARGMIN / ARGMAX tables take mb200_gb_accumulate_arg");
+  if (t->m2_filled) return fail("mb200_gb_accumulate", "a VAR table takes no rows after mb200_gb_accumulate_m2");
   if (int rc = gb_launch(t, reinterpret_cast<const long long*>(keys), vals, nullptr, nullptr, nrows, false,
                          (cudaStream_t)stream))
     return rc;
@@ -1670,6 +1898,7 @@ extern "C" int mb200_gb_merge_partial(mb200_gb_table* t, const int64_t* keys, co
   if (npartial < 0) return fail("mb200_gb_merge_partial", "negative npartial");
   if (npartial > 0 && !keys) return fail("mb200_gb_merge_partial", "null keys");
   if (t->flags & kGbArg) return fail("mb200_gb_merge_partial", "ARGMIN / ARGMAX tables do not merge partial tables");
+  if (t->m2_filled) return fail("mb200_gb_merge_partial", "a VAR table takes no rows after mb200_gb_accumulate_m2");
   return gb_launch(t, reinterpret_cast<const long long*>(keys), sums, cnts, reinterpret_cast<const long long*>(sizes),
                    npartial, true, (cudaStream_t)stream);
 }
@@ -1686,6 +1915,21 @@ extern "C" int mb200_gb_accumulate_arg(mb200_gb_table* t, const int64_t* keys, c
     return rc;
   t->arg_filled = 1;
   t->rows = nrows;
+  return 0;
+}
+
+extern "C" int mb200_gb_accumulate_m2(mb200_gb_table* t, const int64_t* keys, const void* const* vals,
+                                      const void* const* cnts, const void* const* m2s, int64_t nrows,
+                                      mb200_stream_t stream) {
+  if (!t) return fail("mb200_gb_accumulate_m2", "null table");
+  if (!(t->flags & MB200_GB_VAR)) return fail("mb200_gb_accumulate_m2", "not a VAR table");
+  if (nrows < 0) return fail("mb200_gb_accumulate_m2", "negative nrows");
+  if (nrows > 0 && !keys) return fail("mb200_gb_accumulate_m2", "null keys");
+  if (nrows > 0 && t->nvals > 0 && !vals) return fail("mb200_gb_accumulate_m2", "null value columns");
+  if (nrows > 0 && t->nvals > 0 && cnts && !m2s) return fail("mb200_gb_accumulate_m2", "partial rows need M2 columns");
+  if (int rc = gb_var_launch(t, reinterpret_cast<const long long*>(keys), vals, cnts, m2s, nrows, (cudaStream_t)stream))
+    return rc;
+  t->m2_filled = 1;
   return 0;
 }
 
@@ -1816,6 +2060,7 @@ static int gb_emit_impl(mb200_gb_table* t, int64_t ngroups, int sort, int64_t* o
   p.acc = t->acc;
   p.cnt = t->cnt;
   p.size = t->size;
+  p.m2 = t->m2;
   p.nvals = t->nvals;
   p.vstride = t->vstride;
   p.flags = t->flags;
@@ -1824,6 +2069,7 @@ static int gb_emit_impl(mb200_gb_table* t, int64_t ngroups, int sort, int64_t* o
   for (int v = 0; v < t->nvals; ++v) {
     p.out_sums[v] = out_sums ? out_sums[v] : nullptr;
     p.out_cnts[v] = out_cnts ? out_cnts[v] : nullptr;
+    p.out_m2[v] = (out_sums && t->m2) ? out_sums[t->nvals + v] : nullptr;  // a VAR table's out_sums: sums, then M2s
   }
   p.out_sizes = reinterpret_cast<long long*>(out_sizes);
   gb_emit_kernel<<<(unsigned)((ngroups + 255) / 256), 256, 0, st>>>(p);

@@ -1284,14 +1284,21 @@ _PARTIALS = {
     # they came from (``_arg_partial``); the table behind it holds row positions, so partials are never merged as tables
     "idxmax": _Partial(_lib.GB_ARGMAX, ("sums", "labels")),
     "idxmin": _Partial(_lib.GB_ARGMIN, ("sums", "labels")),
+    # var / std: the group sums and counts (pass 1) and the sums of squared deviations from the group means (pass 2);
+    # partials merge pairwise, and the variance M2 / (count - ddof) is taken in DevGroupbyReduce._finalize
+    "var": _Partial(_lib.GB_SUM | _lib.GB_COUNT | _lib.GB_VAR, ("sums", "cnts", "m2")),
+    "std": _Partial(_lib.GB_SUM | _lib.GB_COUNT | _lib.GB_VAR, ("sums", "cnts", "m2")),
 }
 _POSITION_AGGS = ("first", "last")
 _ARG_AGGS = ("idxmax", "idxmin")
+_VAR_AGGS = ("var", "std")
 
 
 def _partial_cols(agg, sums, cnts, sizes):
-    """The emitted arrays of a table in the partial layout of ``agg``."""
+    """The emitted arrays of a table in the partial layout of ``agg`` (a var / std table emits its M2s after its sums)."""
     got = {"sums": sums, "cnts": cnts, "sizes": [sizes]}
+    if agg in _VAR_AGGS:
+        got["sums"], got["m2"] = sums[: len(cnts)], sums[len(cnts) :]
     return [c for name in _PARTIALS[agg].arrays for c in got[name]]
 
 
@@ -1301,7 +1308,7 @@ def _partial_labels(agg, labels):
         return pandas.Index(["size"])
     if len(arrays) == 1:
         return labels
-    tags = {"sums": "sum", "cnts": "count", "labels": "label"}
+    tags = {"sums": "sum", "cnts": "count", "labels": "label", "m2": "m2"}
     return pandas.MultiIndex.from_tuples([(tags[name], c) for name in arrays for c in labels])
 
 
@@ -1339,11 +1346,12 @@ def _split_key_values(block: DeviceBlock, by_block: Optional[DeviceBlock], who: 
 
 
 def _aggregated_values(agg, vals):
-    """The value columns ``agg`` aggregates: none for size, float64 images for count / mean (the table counts non-NaN
-    float64 values); the others take float64 columns only."""
+    """The value columns ``agg`` aggregates: none for size, float64 images for count / mean / var / std (the table
+    counts non-NaN float64 values; pandas casts int64 and bool columns to float64 for these); the others take float64
+    columns only."""
     if agg == "size":
         return []
-    vals = ops.cast_columns_f64(vals) if agg in ("count", "mean") else vals
+    vals = ops.cast_columns_f64(vals) if agg in ("count", "mean", "var", "std") else vals
     if any(v.dtype != np.float64 for v in vals):
         raise NotImplementedError(f"device groupby.{agg} aggregates float64 value columns only")
     return vals
@@ -1494,11 +1502,12 @@ class DevGroupbyReduce(DevFn):
     what the ranks send in rank order -- and on a NaN partial meaning "no value in that partition", exactly as a NaN
     row does (under ``skipna=False`` every column takes the group's first / last partial row)."""
 
-    def __init__(self, agg: str, skipna: bool = True, nan_key: bool = False):
+    def __init__(self, agg: str, skipna: bool = True, nan_key: bool = False, ddof=1):
         self.agg = agg
         self.op = f"groupby_{agg}_reduce"
         self.skipna = skipna
         self.nan_key = nan_key
+        self.ddof = ddof  # var / std only
 
     def _merge(self, keys, cols):
         """Regroup partial rows by key -> ascending unique keys + merged partial columns (same layout as the input).
@@ -1517,6 +1526,8 @@ class DevGroupbyReduce(DevFn):
         W = len(cols) // len(layout.arrays)
         got = {name: list(cols[i * W : (i + 1) * W]) for i, name in enumerate(layout.arrays)}
         sums, cnts, sizes = got.get("sums"), got.get("cnts"), got.get("sizes", [None])[0]
+        if "m2" in got:  # var / std partials go into the table as their emit left them: sums, then M2s
+            sums = sums + got["m2"]
         if sums is None:
             # partial counts are merged through the count accumulators, which want value columns (ignored)
             sums = ops.cast_columns_f64(cnts) if cnts is not None else []
@@ -1527,6 +1538,16 @@ class DevGroupbyReduce(DevFn):
         if self.agg in _ARG_AGGS:
             W = len(cols) // 2
             return _group_block(cols[W:], pandas.Index([t[1] for t in columns[W:]]), k, key_label)
+        if self.agg in _VAR_AGGS:
+            # M2 / (count - ddof), NaN where count <= ddof (pandas' group_var), on the device; std is its square root
+            t = ops.torch_mod()
+            W = len(cols) // 3
+            out = []
+            for s, m2 in zip(cols[W : 2 * W], cols[2 * W :]):
+                d = s.data.to(t.float64) - float(self.ddof)
+                v = t.where(d > 0, m2.data / d, t.full_like(d, float("nan")))
+                out.append(DeviceColumn(t.sqrt(v) if self.agg == "std" else v, np.float64))
+            return _group_block(out, pandas.Index([t_[1] for t_ in columns[:W]]), k, key_label)
         labels = pandas.Index([t[1] for t in columns[: len(cols) // 2]]) if self.agg == "mean" else columns
         return _finished_block(self.agg, k, key_label, cols, labels)
 
@@ -1597,9 +1618,10 @@ def fused_dense_groupby(map_fn: "DevGroupbyMap", reduce_fn: "DevGroupbyReduce", 
     agg = map_fn.agg
     if agg != reduce_fn.agg or not blocks or len(blocks) != len(by_blocks):
         return None
-    if agg in _POSITION_AGGS or agg in _ARG_AGGS:
-        # merging position tables across GPUs would need the values gathered across GPUs too: the general path
-        # (still one dense table per partition when the key range allows) does first / last / idxmax / idxmin
+    if agg in _POSITION_AGGS or agg in _ARG_AGGS or agg in _VAR_AGGS:
+        # merging position tables across GPUs would need the values gathered across GPUs too, and M2s do not merge
+        # element-wise: the general path (still one dense table per partition when the key range allows) does first /
+        # last / idxmax / idxmin / var / std
         return None
     inputs = [_split_key_values(block, by_block, map_fn.op) for block, by_block in zip(blocks, by_blocks)]
     key_label, labels = inputs[0][1], (inputs[0][3] if agg != "size" else inputs[0][3][:0])

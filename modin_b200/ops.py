@@ -378,6 +378,17 @@ class GroupTable:
         with _timed("gb_accumulate"):
             _lib.check(self.lib.mb200_gb_accumulate(self.handle, keys.ptr, ptrs, len(keys), current_stream()))
 
+    def accumulate_m2(self, keys: DeviceColumn, vals: Sequence[DeviceColumn], cnts=None, m2s=None):
+        """Pass 2 of a var / std table (mb200_gb_accumulate_m2), after every pass-1 call: add each value's squared
+        deviation from its group's mean into the table's M2s.  Raw float64 rows ``vals``, or with ``cnts`` / ``m2s`` the
+        emitted sums, counts and M2s of other var / std tables.  The table takes no pass-1 rows afterwards."""
+        if any(v.dtype != np.float64 for v in vals):
+            raise TypeError("device groupby.var / std aggregate float64 value columns")
+        ptrs = lambda cols: _lib.ptr_array([c.ptr for c in cols]) if cols is not None else None  # noqa: E731
+        with _timed("gb_accumulate_m2"):
+            _lib.check(self.lib.mb200_gb_accumulate_m2(self.handle, keys.ptr, ptrs(vals), ptrs(cnts), ptrs(m2s), len(keys),
+                                                       current_stream()))  # fmt: skip
+
     def merge_partial(self, keys: DeviceColumn, sums, cnts=None, sizes: Optional[DeviceColumn] = None):
         ps = _lib.ptr_array([v.ptr for v in sums]) if sums else None
         pc = _lib.ptr_array([v.ptr for v in cnts]) if cnts else None
@@ -395,7 +406,8 @@ class GroupTable:
     def _outputs(self, rows: int):
         """Empty (keys, sums, cnts, sizes) columns of ``rows`` rows for what this table emits."""
         acc_dtype = np.int64 if self.flags & _GB_POS else np.float64  # first / last / idxmin / idxmax emit row positions
-        sums = [DeviceColumn.empty(rows, acc_dtype) for _ in range(self.nvals)] if self.flags & _GB_ACC else None
+        nsums = 2 * self.nvals if self.flags & _lib.GB_VAR else self.nvals  # var / std: the sums, then the M2s
+        sums = [DeviceColumn.empty(rows, acc_dtype) for _ in range(nsums)] if self.flags & _GB_ACC else None
         cnts = [DeviceColumn.empty(rows, np.int64) for _ in range(self.nvals)] if self.flags & _lib.GB_COUNT else None
         sizes = DeviceColumn.empty(rows, np.int64) if self.flags & _lib.GB_SIZE else None
         return DeviceColumn.empty(rows, np.int64), sums, cnts, sizes
@@ -445,16 +457,29 @@ class GroupTable:
             pass
 
 
-# The table driver works through the table's library calls only (accumulate / merge_partial / ngroups / emit), so that
-# whatever stands in for a table needs nothing else.
+# The table driver works through the table's library calls only (accumulate / merge_partial / accumulate_m2 / ngroups /
+# emit), so that whatever stands in for a table needs nothing else.
 def fill_table(table, items, partial: bool = False):
     """Aggregate every input into ``table``: raw ``(keys, vals)`` rows (``accumulate``), or with ``partial`` the
-    emitted ``(keys, sums, cnts, sizes)`` of other tables (``merge_partial``).  Returns the table."""
+    emitted ``(keys, sums, cnts, sizes)`` of other tables (``merge_partial``).  A var / std table's partial ``sums``
+    hold the sums, then the M2s, as its emit does; once every input has set the group means (pass 1), every input
+    goes through ``accumulate_m2`` (pass 2).  Returns the table."""
+    var = table.flags & _lib.GB_VAR
     for item in items:
-        if partial:
+        if partial and var:
+            W = len(item[2])
+            table.merge_partial(item[0], item[1][:W], item[2], *item[3:])
+        elif partial:
             table.merge_partial(*item)
         else:
             table.accumulate(item[0], item[1])
+    if var:
+        for item in items:
+            if partial:
+                W = len(item[2])
+                table.accumulate_m2(item[0], item[1][:W], item[2], item[1][W:])
+            else:
+                table.accumulate_m2(item[0], item[1])
     return table
 
 
@@ -538,7 +563,7 @@ def dense_range_ok(lo: int, hi: int, cap: int, total_rows: int, nvals: int, flag
     rng = hi - lo + 1
     if rng > (1 << 29) or rng > max(4 * cap, total_rows // 2, 1 << 16):
         return False
-    arrays = (1 if flags & _GB_ACC else 0) + (1 if flags & _GB_CNT else 0)
+    arrays = (1 if flags & _GB_ACC else 0) + (1 if flags & _GB_CNT else 0) + (1 if flags & _lib.GB_VAR else 0)
     return rng * (value_stride(nvals) * 8 * arrays + 9) <= DENSE_TABLE_MAX_BYTES
 
 
@@ -614,17 +639,29 @@ def plan_table(key_cols: Sequence[DeviceColumn], nvals: int, flags: int, capacit
 def hash_aggregate(key_cols_vals, flags: int, capacity_hint: int, partial: bool = False, sort: bool = True):
     """Aggregate a list of (keys, vals[, cnts, sizes]) inputs into one table and emit it: a dense
     (direct-addressed) table when the key range allows, else the hash table, grown when it
-    overflows.  Returns (keys, sums, cnts, sizes) device columns."""
-    nvals = len(key_cols_vals[0][1]) if key_cols_vals[0][1] else 0
+    overflows.  Returns (keys, sums, cnts, sizes) device columns.  A var / std table's sums are the sums, then the M2s
+    (2 x nvals columns), in its partial inputs and in its result alike."""
+    halves = 2 if partial and flags & _lib.GB_VAR else 1
+    nvals = (len(key_cols_vals[0][1]) if key_cols_vals[0][1] else 0) // halves
     if nvals > _lib.MAX_COLS:
         # a table holds at most MAX_COLS value columns: aggregate them MAX_COLS at a time.  Every pass sees the same
-        # keys, so every table holds the same groups; emitted in ascending key order, their rows line up.
+        # keys, so every table holds the same groups; emitted in ascending key order, their rows line up.  Lists of
+        # several nvals-long runs (a var / std table's sums, then M2s) are cut and joined run by run.
+        def cut(cols, k):
+            if not cols:
+                return cols
+            return [c for h in range(0, len(cols), nvals) for c in cols[h + k : h + min(k + _lib.MAX_COLS, nvals)]]
+
+        def join(lists):
+            if lists[0] is None:
+                return None
+            runs = len(lists[0]) // min(_lib.MAX_COLS, nvals)
+            return [c for r in range(runs) for cs in lists for c in cs[r * (len(cs) // runs) : (r + 1) * (len(cs) // runs)]]
+
         parts = []
         for k in range(0, nvals, _lib.MAX_COLS):
-            cut = lambda cols: cols[k : k + _lib.MAX_COLS] if cols else cols  # noqa: E731
-            items = [(it[0], cut(it[1])) + ((cut(it[2]),) + tuple(it[3:]) if len(it) > 2 else ()) for it in key_cols_vals]
+            items = [(it[0], cut(it[1], k)) + ((cut(it[2], k),) + tuple(it[3:]) if len(it) > 2 else ()) for it in key_cols_vals]
             parts.append(hash_aggregate(items, flags, capacity_hint, partial=partial, sort=True))
-        join = lambda cols: [c for cs in cols for c in cs] if cols[0] is not None else None  # noqa: E731
         return parts[0][0], join([p[1] for p in parts]), join([p[2] for p in parts]), parts[0][3]
     plan = plan_table([item[0] for item in key_cols_vals], nvals, flags, capacity_hint, partial=partial)
     cap = plan.capacity

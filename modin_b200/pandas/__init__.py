@@ -635,11 +635,25 @@ class DataFrameGroupBy:
         return self._wrap_aggregation(type(self._query_compiler).groupby_idxmin, numeric_only,
                                       agg_kwargs=dict(axis=0, skipna=skipna))  # fmt: skip
 
+    def var(self, ddof=1, engine=None, engine_kwargs=None, numeric_only=False):
+        """The sample variance of every column per group (NaN skipped; NaN where a group has ``ddof`` values or
+        fewer), passed on as modin/pandas/groupby.py:1264-1278 does.  Only pandas' own engine."""
+        if engine not in ("cython", None) or engine_kwargs is not None:
+            raise NotImplementedError(f"groupby.var(engine={engine!r}) is not on the B200 path")
+        return self._wrap_aggregation(type(self._query_compiler).groupby_var, numeric_only, agg_kwargs=dict(ddof=ddof))
+
+    def std(self, ddof=1, engine=None, engine_kwargs=None, numeric_only=False):
+        if engine not in ("cython", None) or engine_kwargs is not None:
+            raise NotImplementedError(f"groupby.std(engine={engine!r}) is not on the B200 path")
+        return self._wrap_aggregation(type(self._query_compiler).groupby_std, numeric_only, agg_kwargs=dict(ddof=ddof))
+
     def size(self):
         res = self._wrap_aggregation(type(self._query_compiler).groupby_size)
         return Series(query_compiler=res._query_compiler)
 
     def agg(self, func, *args, **kwargs):
+        if isinstance(func, str) and func in ("var", "std") and not args:
+            return getattr(self, func)(**kwargs)
         if isinstance(func, str) and func in ("sum", "count", "mean", "size", "min", "max", "first", "last", "idxmax",
                                                  "idxmin"):
             return getattr(self, func)()

@@ -85,11 +85,28 @@ def _arg_agg_kwargs(agg: str, agg_kwargs) -> None:
         raise NotImplementedError(f"groupby.{agg}(axis={axis!r}) is not on the B200 path")
 
 
+def _var_ddof(agg: str, agg_kwargs):
+    """``ddof`` of ``groupby.var`` / ``std`` from the ``agg_kwargs`` Modin passes (modin/pandas/groupby.py:1264-1278),
+    truncated towards zero as pandas does.  ``numeric_only`` is dropped (the caller has selected the columns); any
+    other argument, such as another engine, is refused."""
+    kw = dict(agg_kwargs or {})
+    ddof = kw.pop("ddof", 1)
+    kw.pop("numeric_only", None)
+    if kw.get("engine") in ("cython", None) and kw.get("engine_kwargs") is None:  # pandas' own engine
+        kw.pop("engine", None)
+        kw.pop("engine_kwargs", None)
+    if kw:
+        raise NotImplementedError(f"groupby.{agg}({', '.join(kw)}=) is not on the B200 path")
+    if not isinstance(ddof, (int, float, np.integer, np.floating)):
+        raise TypeError(f"ddof must be a number, got {ddof!r}")
+    return int(ddof)  # pandas 3.0.2's group_var takes ddof as an integer: 1.5 acts as 1, -0.5 as 0
+
+
 def _groupby_reduce(agg: str):
     """``qc.groupby_<agg>`` (qc.py:3741-3748, alg/groupby.py) over device blocks.  ``by`` is a query compiler of key
     columns with the frame's rows; ``key_names`` replaces the names of the result's keys (``groupby(level=)``).
-    ``agg_kwargs`` are read by first / last (``skipna``, ``min_count``) and idxmax / idxmin (``skipna``, ``axis``) only;
-    the other aggregations ignore them."""
+    ``agg_kwargs`` are read by first / last (``skipna``, ``min_count``), idxmax / idxmin (``skipna``, ``axis``) and
+    var / std (``ddof``) only; the other aggregations ignore them."""
     map_f, red_f = DevGroupbyMap(agg), DevGroupbyReduce(agg)
 
     def caller(query_compiler, by, axis, groupby_kwargs, agg_args, agg_kwargs, drop=False, key_names=None, **kwargs):
@@ -105,6 +122,8 @@ def _groupby_reduce(agg: str):
             fns = (DevGroupbyMap(agg, skipna=skipna), DevGroupbyReduce(agg, skipna=skipna))
         if agg in ("idxmax", "idxmin"):
             _arg_agg_kwargs(agg, agg_kwargs)
+        if agg in ("var", "std"):
+            fns = (map_f, DevGroupbyReduce(agg, ddof=_var_ddof(agg, agg_kwargs)))
         frame, by_frame = query_compiler._modin_frame, by._modin_frame
         # a float64 key or several int64 keys: the single-key groupby runs on their int64 image and the G result keys
         # are restored afterwards (groupkeys.py); one int64 key is its own image
@@ -239,8 +258,11 @@ def device_operations(alg):
         groupby_last = _groupby_reduce("last")
         groupby_idxmax = _groupby_reduce("idxmax")
         groupby_idxmin = _groupby_reduce("idxmin")
+        groupby_var = _groupby_reduce("var")
+        groupby_std = _groupby_reduce("std")
 
-        _DEVICE_AGGS = ("sum", "count", "size", "mean", "min", "max", "first", "last", "idxmax", "idxmin")
+        _DEVICE_AGGS = ("sum", "count", "size", "mean", "min", "max", "first", "last", "idxmax", "idxmin", "var", "std")
+        _KWARG_AGGS = ("first", "last", "idxmax", "idxmin", "var", "std")  # aggregations that read agg_kwargs
 
         def groupby_agg(self, by, agg_func, axis, groupby_kwargs, agg_args, agg_kwargs, how="axis_wise", drop=False,
                         series_groupby=False):  # fmt: skip
@@ -251,7 +273,7 @@ def device_operations(alg):
             ask for it; every result carries the same ascending group keys, so the result blocks are zipped
             column-wise (buffers shared) in the dictionary's order.  A function name alone goes to its registered
             template.  Anything else has no device form and is refused -- there is no pandas block to fall back to."""
-            if how != "axis_wise" or agg_args or (agg_kwargs and agg_func not in ("first", "last", "idxmax", "idxmin")):
+            if how != "axis_wise" or agg_args or (agg_kwargs and agg_func not in self._KWARG_AGGS):
                 raise NotImplementedError(f"groupby ({how}) with extra arguments is not on the B200 path")
             if isinstance(agg_func, str) and agg_func in self._DEVICE_AGGS:
                 return getattr(self, f"groupby_{agg_func}")(
@@ -263,11 +285,12 @@ def device_operations(alg):
                 raise NotImplementedError("device groupby: key columns of the same frame, axis=0")
             spec = {col: fn[0] if isinstance(fn, (list, tuple)) and len(fn) == 1 else fn for col, fn in agg_func.items()}
             by_func = gk.split_aggregations(spec, self.columns, set(by.columns) if drop else ())
-            if len(by_func) > 1 and set(by_func) & {"first", "last", "idxmax", "idxmin"} and dist.is_distributed():
+            if len(by_func) > 1 and set(by_func) & {"first", "last", "idxmax", "idxmin", "var", "std"} \
+                    and dist.is_distributed():  # fmt: skip
                 # across ranks the fused dense path of the other functions and the key-range exchange of first / last /
-                # idxmax / idxmin give each rank a different key range
-                raise NotImplementedError("groupby.agg mixing first / last / idxmax / idxmin with other functions "
-                                          "across ranks")  # fmt: skip
+                # idxmax / idxmin / var / std give each rank a different key range
+                raise NotImplementedError("groupby.agg mixing first / last / idxmax / idxmin / var / std with other "
+                                          "functions across ranks")  # fmt: skip
             if any(isinstance(fn, (list, tuple)) for fn in agg_func.values()):
                 raise NotImplementedError("groupby.agg with lists of functions (two-level result columns)")
             kw = dict(groupby_kwargs, as_index=True)
