@@ -40,8 +40,10 @@ extern "C" {
 /* 2: round 2 (key statistics, async dense emit, expand / concat / comm entry points); 3: + the Fold template's
  * cumulative scans (mb200_cum_*); 4: + MB200_GB_FIRST / MB200_GB_LAST group tables (row positions, NULL value
  * columns); 5: + MB200_GB_ARGMIN / MB200_GB_ARGMAX group tables and mb200_gb_accumulate_arg; 6: + MB200_GB_VAR group
- * tables and mb200_gb_accumulate_m2.  Checked by the binding at load time (modin_b200/_lib.py). */
-#define MB200_ABI_VERSION 6
+ * tables and mb200_gb_accumulate_m2; 7: + MB200_GB_NUNIQUE group tables, their distinct set and
+ * mb200_gb_reserve_distinct / mb200_gb_accumulate_distinct / mb200_gb_emit_distinct.  Checked by the binding at load
+ * time (modin_b200/_lib.py). */
+#define MB200_ABI_VERSION 7
 #define MB200_MAX_COLS 32 /* max columns per launch == Modin's MinColumnPartitionSize (envvars.py:1149-1190) */
 
 typedef void* mb200_stream_t;
@@ -145,7 +147,12 @@ enum mb200_gb_flags {
    * library allocates for dense tables too (it is not among the caller-owned arrays of mb200_gb_create_dense) and
    * which starts at 0.  Pass 1 fills acc / cnt (mb200_gb_accumulate, mb200_gb_merge_partial); pass 2 fills m2
    * (mb200_gb_accumulate_m2) */
-  MB200_GB_VAR = 512
+  MB200_GB_VAR = 512,
+  /* groupby.nunique: a NUNIQUE table is exactly SIZE | NUNIQUE.  cnt[g][v] holds the number of distinct values of
+   * column v in group g, from 0.  Pass 1 (mb200_gb_accumulate / mb200_gb_merge_partial) is the SIZE launch: it inserts
+   * the groups and reads no value column.  Pass 2 (mb200_gb_accumulate_distinct) inserts (group, column, value image)
+   * entries into the table's distinct set (mb200_gb_reserve_distinct) and counts the new ones into cnt */
+  MB200_GB_NUNIQUE = 1024
 };
 
 /* ======================= runtime / memory ================================== */
@@ -296,6 +303,29 @@ int mb200_gb_accumulate_arg(mb200_gb_table* table, const int64_t* keys, const vo
  * run-dependent, the result is within the bound stated in README.md, not bit for bit. */
 int mb200_gb_accumulate_m2(mb200_gb_table* table, const int64_t* keys, const void* const* vals,
                            const void* const* cnts, const void* const* m2s, int64_t nrows, mb200_stream_t stream);
+/* The distinct set of a NUNIQUE table: open addressing over `capacity` (a power of two, at most 2^32) 16-byte slots
+ * {int64 entry = gid * vstride + column, int64 image}, empty = {-1, 0}, in library-owned memory.  Allocates the set,
+ * or clears it for reuse when it is already at least that large.  Must be called before mb200_gb_accumulate_distinct. */
+int mb200_gb_reserve_distinct(mb200_gb_table* table, int64_t capacity, mb200_stream_t stream);
+/* Pass 2 of a NUNIQUE table (groupby.nunique), after every pass-1 call.  Each (group, column, image) entry that is not
+ * in the set yet is inserted and adds 1 to cnt[gid][column]; keys that are not in the table add nothing.  Images: a
+ * float64 value's order-preserving int64 image with -0.0 folded into +0.0 and every NaN mapped to one image; an int64
+ * value itself (bool columns are widened to int64 by the caller).
+ * Raw form (col_ids == NULL): vals[nvals][nrows], column v int64 iff bit v of i64_mask is set; NaN is skipped iff
+ * dropna.  Partial form (col_ids != NULL): the rows of other NUNIQUE tables' mb200_gb_emit_distinct, col_ids[nrows] and
+ * images[nrows] (int64); a row with column id -1 carries its group only.  A full set raises the table's overflow flag
+ * (mb200_gb_ngroups reports it).  The counts are exact whatever the order of the atomics. */
+int mb200_gb_accumulate_distinct(mb200_gb_table* table, const int64_t* keys, const void* const* vals, uint32_t i64_mask,
+                                 int dropna, const int64_t* col_ids, const int64_t* images, int64_t nrows,
+                                 mb200_stream_t stream);
+/* The distinct set of a NUNIQUE table as rows for another table's partial pass 2: out_keys / out_cols / out_images
+ * [capacity] (int64) take one (key, -1, 0) row per group of the table, then one (key, column, image) row per entry, in
+ * no particular order.  `ngroups` as reported by mb200_gb_ngroups.  The number of rows is decided on the device and
+ * left, with an overflow flag (rows beyond `capacity`), in count_overflow_dev[2] (device int64).  Scratch as for
+ * mb200_gb_emit(ngroups). */
+int mb200_gb_emit_distinct(mb200_gb_table* table, int64_t ngroups, int64_t capacity, int64_t* out_keys,
+                           int64_t* out_cols, int64_t* out_images, void* scratch, int64_t* count_overflow_dev,
+                           mb200_stream_t stream);
 /* Synchronises `stream`; returns number of groups and whether capacity was exceeded. */
 int mb200_gb_ngroups(mb200_gb_table* table, int64_t* ngroups, int* overflow,
                      mb200_stream_t stream);
@@ -305,7 +335,8 @@ size_t mb200_gb_emit_scratch_bytes(int64_t ngroups);
  * out_cnts[nvals][ngroups] (int64, may be NULL), out_sizes[ngroups] (may be NULL).
  * FIRST / LAST and ARGMIN / ARGMAX tables write int64 positions into out_sums, -1 where the group has no non-NaN
  * value in the column (mb200_take turns -1 into NaN).  A VAR table's out_sums holds 2 * nvals pointers: the sums
- * out_sums[0 .. nvals), then the M2s out_sums[nvals .. 2 nvals) (float64; an entry may be NULL). */
+ * out_sums[0 .. nvals), then the M2s out_sums[nvals .. 2 nvals) (float64; an entry may be NULL).  A NUNIQUE table
+ * writes its distinct counts into out_cnts. */
 int mb200_gb_emit(mb200_gb_table* table, int64_t ngroups, int sort, int64_t* out_keys,
                   void* const* out_sums, void* const* out_cnts, int64_t* out_sizes,
                   void* scratch, mb200_stream_t stream);

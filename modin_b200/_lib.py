@@ -20,7 +20,7 @@ class B200Error(RuntimeError):
     """Raised when a libmodin_b200 call fails (message from mb200_last_error)."""
 
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 # enums (keep in sync with include/modin_b200.h)
 F64, I64, U8 = 0, 1, 2
@@ -43,6 +43,7 @@ GB_SUM, GB_COUNT, GB_SIZE, GB_MIN, GB_MAX = 1, 2, 4, 8, 16
 GB_FIRST, GB_LAST = 32, 64  # int64 row positions instead of values (include/modin_b200.h)
 GB_ARGMIN, GB_ARGMAX = 128, 256  # the first row holding each group's extreme (mb200_gb_accumulate_arg)
 GB_VAR = 512  # SUM | COUNT | VAR: sums of squared deviations from the group means (mb200_gb_accumulate_m2)
+GB_NUNIQUE = 1024  # SIZE | NUNIQUE: distinct counts through the table's distinct set (mb200_gb_accumulate_distinct)
 
 _vp = C.c_void_p
 _vpp = C.POINTER(C.c_void_p)
@@ -84,6 +85,9 @@ _SIGNATURES = {
     "mb200_gb_accumulate_arg": (C.c_int, [_vp, _vp, _vpp, C.c_uint32, _i64, _vp]),
     "mb200_gb_merge_partial": (C.c_int, [_vp, _vp, _vpp, _vpp, _vp, _i64, _vp]),
     "mb200_gb_accumulate_m2": (C.c_int, [_vp, _vp, _vpp, _vpp, _vpp, _i64, _vp]),
+    "mb200_gb_reserve_distinct": (C.c_int, [_vp, _i64, _vp]),
+    "mb200_gb_accumulate_distinct": (C.c_int, [_vp, _vp, _vpp, C.c_uint32, C.c_int, _vp, _vp, _i64, _vp]),
+    "mb200_gb_emit_distinct": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mb200_gb_ngroups": (C.c_int, [_vp, C.POINTER(_i64), C.POINTER(C.c_int), _vp]),
     "mb200_gb_emit_scratch_bytes": (C.c_size_t, [_i64]),
     "mb200_gb_emit": (C.c_int, [_vp, _i64, C.c_int, _vp, _vpp, _vpp, _vp, _vp, _vp]),

@@ -122,3 +122,12 @@ class GroupbyAsyncEmit(Parameter):
     varname = "MB200_GB_ASYNC_EMIT"
     default = True
     type = bool
+
+
+class GroupbyDistinctBytes(Parameter):
+    """Device bytes one column batch of ``groupby.nunique`` may give its distinct set (16 B per slot, at least twice as
+    many slots as the batch has values).  Wider frames run in more batches, each with its own pass over the keys; one
+    column always runs, even when its set alone is larger."""
+
+    varname = "MB200_GB_DISTINCT_BYTES"
+    default = 8 << 30

@@ -50,6 +50,12 @@ struct __align__(16) Slot {
   int pad;
 };
 
+// one entry of a NUNIQUE table's distinct set: (gid * vstride + column, value image); empty = {-1, 0}
+struct __align__(16) DSlot {
+  long long entry;
+  long long image;
+};
+
 struct GbMeta {  // device-side bookkeeping
   int ngroups;
   int overflow;
@@ -89,6 +95,10 @@ struct mb200_gb_table {
   int arg_filled;  // ARGMIN / ARGMAX: mb200_gb_accumulate_arg has run (it runs once per table)
   double* m2;      // VAR: sums of squared deviations [gcap][vstride], always the library's (in the arena when hashed)
   int m2_filled;   // VAR: mb200_gb_accumulate_m2 has run, so the means are final and pass-1 calls are refused
+  // NUNIQUE: the distinct set, `dcap` slots in use (a power of two) of an allocation of `dset_alloc` slots
+  mb200::DSlot* dset;
+  long long dcap, dset_alloc;
+  int distinct_filled;  // NUNIQUE: mb200_gb_accumulate_distinct has run, so pass-1 calls are refused
 };
 
 namespace mb200 {
@@ -97,6 +107,7 @@ constexpr int kGbThreads = 256;
 constexpr int kGbWarps = kGbThreads / 32;
 constexpr int kGbArg = MB200_GB_ARGMIN | MB200_GB_ARGMAX;  // groupby.idxmin / idxmax tables
 constexpr int kGbVarTable = MB200_GB_SUM | MB200_GB_COUNT | MB200_GB_VAR;  // groupby.var / std: the only VAR combination
+constexpr int kGbNuniqueTable = MB200_GB_SIZE | MB200_GB_NUNIQUE;  // groupby.nunique: the only NUNIQUE combination
 constexpr int kColStride = 34;  // doubles; 34 = 2 (mod 16) -> conflict-free transposed reads
 // TMA-staged kernel
 constexpr int kTileRows = 256;
@@ -959,7 +970,8 @@ static long long next_pow2(long long v) {
 //        from -0.0, the one value no sum can end on (x + -0.0 = x, and the emit turns it into +0.0), so that a key whose
 //        accumulators moved is present; hashed sums from 0.  Min, FIRST and ARG positions start from INT64_MAX, max and
 //        LAST from INT64_MIN.
-//   cnt: non-NaN counts from 0, or an ARG table's extreme images: from INT64_MIN for ARGMAX, INT64_MAX for ARGMIN.
+//   cnt: non-NaN counts from 0, a NUNIQUE table's distinct counts from 0, or an ARG table's extreme images: from
+//        INT64_MIN for ARGMAX, INT64_MAX for ARGMIN.
 //   size: rows per group, from 0.
 //   m2: VAR tables' sums of squared deviations from the group means, float64 from 0.
 struct TableArrays {
@@ -970,7 +982,7 @@ static TableArrays table_arrays(int flags, bool dense) {
   const long long lo = (long long)0x8000000000000000ULL, hi = 0x7fffffffffffffffLL;
   TableArrays a;
   a.acc = flags & (MB200_GB_SUM | MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST | kGbArg);
-  a.cnt = flags & (MB200_GB_COUNT | kGbArg);
+  a.cnt = flags & (MB200_GB_COUNT | kGbArg | MB200_GB_NUNIQUE);
   a.size = flags & MB200_GB_SIZE;
   a.m2 = flags & MB200_GB_VAR;
   a.acc_init = (flags & MB200_GB_SUM) ? (dense ? lo : 0) : (flags & (MB200_GB_MIN | MB200_GB_FIRST | kGbArg)) ? hi : lo;
@@ -1044,7 +1056,8 @@ typedef size_t (*SmemLayoutFn)(const mb200_gb_table* t, int nrep, SmemTableLayou
 
 // accumulate tables: acc replicas (8 B) | cnt replicas (4 B) | size replicas (4 B) | presence bytes
 static size_t smem_layout_accumulate(const mb200_gb_table* t, int nrep, SmemTableLayout* lay) {
-  const TableArrays ta = table_arrays(t->flags, true);
+  // a NUNIQUE table's pass 1 is the SIZE launch: its cnt is pass 2's
+  const TableArrays ta = table_arrays((t->flags & MB200_GB_NUNIQUE) ? MB200_GB_SIZE : t->flags, true);
   lay->svs = t->vstride + 1;
   lay->rstride = (int)((((size_t)t->gcap * lay->svs + 15) & ~(size_t)15) + 1);
   lay->zstride = (int)(t->gcap | 1);
@@ -1096,10 +1109,15 @@ static int gb_launch(mb200_gb_table* t, const long long* keys, const void* const
   DevProps dp;
   if (int rc = dev_props(&dp)) return rc;
   GbParams p = gb_params(t, keys, nrows);
+  if (t->flags & MB200_GB_NUNIQUE) {  // pass 1 of a NUNIQUE table is the groupby.size launch: no value column is read
+    p.nvals = 0;
+    p.cnt = nullptr;
+    p.flags = MB200_GB_SIZE;
+  }
   const bool pos = t->flags & (MB200_GB_FIRST | MB200_GB_LAST);
   if (pos && partial) return fail("groupby", "FIRST / LAST tables do not merge partial tables");
   bool aligned = aligned16(keys);
-  for (int c = 0; c < t->nvals; ++c) {
+  for (int c = 0; c < p.nvals; ++c) {
     p.vals[c] = vals ? vals[c] : nullptr;
     p.pcnt[c] = pcnt ? pcnt[c] : nullptr;
     if ((t->flags & (MB200_GB_SUM | MB200_GB_COUNT | MB200_GB_MIN | MB200_GB_MAX)) && !p.vals[c])
@@ -1174,7 +1192,7 @@ static int gb_launch(mb200_gb_table* t, const long long* keys, const void* const
     MB_LAUNCH_CHECK("gb_accumulate_smem_kernel");
     return 0;
   }
-  if (!gb_direct_only() && !partial && aligned && t->nvals <= 8 && nrows >= kTileRows) {
+  if (!gb_direct_only() && !partial && aligned && p.nvals <= 8 && nrows >= kTileRows) {
     const long long ntiles = nrows / kTileRows;
     const bool hot = t->skewed && !(t->flags & (MB200_GB_MIN | MB200_GB_MAX | MB200_GB_FIRST | MB200_GB_LAST | MB200_GB_SIZE));
     // hashed tables: a 2-stage ring lets 5 CTAs share an SM instead of 4 (the probe chain wants warps, not staging depth)
@@ -1197,7 +1215,7 @@ static int gb_launch(mb200_gb_table* t, const long long* keys, const void* const
     if (done == nrows) return 0;
     // ragged tail (< 256 rows) goes through the direct-load kernel
     p.keys = keys + done;
-    for (int c = 0; c < t->nvals; ++c)
+    for (int c = 0; c < p.nvals; ++c)
       if (p.vals[c]) p.vals[c] = static_cast<const double*>(p.vals[c]) + done;
     p.row0 += done;
     p.nrows = nrows - done;
@@ -1641,6 +1659,241 @@ static int gb_var_launch(mb200_gb_table* t, const long long* keys, const void* c
                  : launch_direct(gb_var_kernel<false>, "gb_var_kernel", p, dp, st, v);
 }
 
+
+// ---------------------------------------------------------------- NUNIQUE tables (groupby.nunique): the distinct set
+// Pass 1 is the SIZE launch (mb200_gb_accumulate / mb200_gb_merge_partial on the kernels above, which never read the
+// NUNIQUE bit): it inserts the groups.  Pass 2 (mb200_gb_accumulate_distinct) inserts one (gid * vstride + column,
+// image) entry per value into the table's open-addressed distinct set; the insert that claims an empty slot adds 1 to
+// cnt at that entry's offset, so every entry is counted exactly once whatever the order of the atomics.
+struct DistinctParams {
+  DSlot* set;
+  unsigned long long mask;      // set capacity - 1 (a power of two)
+  const long long* col_ids;     // PARTIAL: column of each row, -1 = a row that carries its group only
+  const long long* images;      // PARTIAL: the value image of each row
+  unsigned int i64_mask;        // raw: bit v = column v is int64
+  int dropna;                   // raw: skip NaN values
+};
+
+constexpr long long kNanImage = 0x7ff8000000000000LL;  // every NaN: no non-NaN float64 has this image
+
+// image of one raw value; false = skipped (a NaN under dropna)
+__device__ __forceinline__ bool distinct_image(double x, bool i64, bool dropna, long long& img) {
+  if (i64) {
+    img = __double_as_longlong(x);
+    return true;
+  }
+  if (x != x) {
+    img = kNanImage;
+    return !dropna;
+  }
+  img = (x == 0.0) ? 0LL : f64_to_ordered(x);  // -0.0 and 0.0 are one value
+  return true;
+}
+
+__device__ __forceinline__ unsigned long long distinct_hash(long long entry, long long image) {
+  return (unsigned long long)hash_key(image ^ (long long)((unsigned long long)entry * 0x9e3779b97f4a7c15ULL)) |
+         ((unsigned long long)hash_key(entry + image) << 32);
+}
+
+// Insert the active lanes' (entry, image) pairs; called by all 32 lanes.  Lanes holding the same pair probe once (the
+// lowest of them); a probe reads each slot before it CASes, so a value that is already in the set costs a load, not an
+// atomic.  The lanes that claimed slots of the same entry add their count with one RED.
+__device__ __forceinline__ void distinct_insert(const GbParams& p, const DistinctParams& d, bool active, long long entry,
+                                                long long image) {
+  const int lane = threadIdx.x & 31;
+  const long long e = active ? entry : -1;
+  const unsigned int peers = __match_any_sync(0xffffffffu, (unsigned long long)e) &
+                             __match_any_sync(0xffffffffu, (unsigned long long)image);
+  bool claimed = false;
+  if (active && __ffs(peers) - 1 == lane) {
+    const unsigned __int128 empty = (unsigned __int128)(unsigned long long)-1LL;
+    const unsigned __int128 mine =
+        ((unsigned __int128)(unsigned long long)image << 64) | (unsigned __int128)(unsigned long long)entry;
+    unsigned long long s = distinct_hash(entry, image) & d.mask;
+    for (unsigned long long n = 0;; ++n) {
+      if (n > d.mask) {  // every slot holds another entry
+        p.meta->overflow = 1;
+        break;
+      }
+      DSlot* slot = d.set + s;
+      unsigned long long se, si;
+      asm volatile("ld.relaxed.gpu.global.v2.u64 {%0,%1}, [%2];" : "=l"(se), "=l"(si) : "l"(slot) : "memory");
+      if ((long long)se == entry && si != (unsigned long long)image && si == 0ULL) {
+        // {entry, 0} may be a slot whose claim is being written: read it again, whole
+        const unsigned __int128 now = atomicCAS(reinterpret_cast<unsigned __int128*>(slot), empty, empty);
+        se = (unsigned long long)now;
+        si = (unsigned long long)(now >> 64);
+      }
+      if ((long long)se == entry && (long long)si == image) break;  // already counted
+      if ((long long)se == -1LL) {
+        const unsigned __int128 old = atomicCAS(reinterpret_cast<unsigned __int128*>(slot), empty, mine);
+        if (old == empty) {
+          claimed = true;
+          break;
+        }
+        if (old == mine) break;  // another warp inserted the same pair first
+      }
+      s = (s + 1) & d.mask;
+    }
+  }
+  const unsigned int same = __match_any_sync(0xffffffffu, (unsigned long long)(claimed ? entry : -1LL));
+  if (claimed && __ffs(same) - 1 == lane) red_add_u64(p.cnt + entry, (long long)__popc(same));
+}
+
+// Raw: the mapping of gb_var_kernel (warp = 32 rows, value tile transposed through shared memory, 8 lanes on the 8
+// columns of one row).  Partial: one row per lane, one entry per row.
+template <bool PARTIAL>
+__global__ void __launch_bounds__(kGbThreads, 4) gb_distinct_kernel(const __grid_constant__ GbParams p,
+                                                                    const __grid_constant__ DistinctParams d) {
+  __shared__ double s_tile[kGbWarps][8 * kColStride];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long nchunks = (p.nrows + 31) >> 5;
+  const long long wstride = (long long)gridDim.x * kGbWarps;
+  const int gcap = (int)p.gcap;
+  const uint64_t pol = l2_policy_evict_first();
+  for (long long ch = (long long)blockIdx.x * kGbWarps + warp; ch < nchunks; ch += wstride) {
+    const long long base = ch << 5;
+    const long long row = base + lane;
+    const bool valid = row < p.nrows;
+    long long k = valid ? ldg_stream_i64(p.keys + row, pol) : 0;
+    if (PARTIAL) {
+      const long long j = valid ? ldg_stream_i64(d.col_ids + row, pol) : -1;
+      const long long img = valid ? ldg_stream_i64(d.images + row, pol) : 0;
+      const long long k0 = __shfl_sync(0xffffffffu, k, 0);
+      k = valid ? k : k0;
+      const int gid = lookup_gid(p, k);
+      const bool active = valid && gid < gcap && j >= 0 && j < p.nvals;
+      distinct_insert(p, d, active, (long long)gid * p.vstride + j, img);
+      continue;
+    }
+    double x[8];
+    {
+      const int nc = p.nvals < 8 ? p.nvals : 8;
+#pragma unroll
+      for (int c = 0; c < 8; ++c)
+        x[c] = (c < nc && valid) ? ldg_stream_f64(static_cast<const double*>(p.vals[c]) + row, pol) : 0.0;
+    }
+    {
+      const long long k0 = __shfl_sync(0xffffffffu, k, 0);  // rows past the end join lane 0's peer group
+      k = valid ? k : k0;
+    }
+    const int gid = lookup_gid(p, k);
+    for (int c0 = 0; c0 < p.nvals; c0 += 8) {
+      const int nc = (p.nvals - c0) < 8 ? (p.nvals - c0) : 8;
+      if (c0 > 0) {
+#pragma unroll
+        for (int c = 0; c < 8; ++c)
+          x[c] = (c < nc && valid) ? ldg_stream_f64(static_cast<const double*>(p.vals[c0 + c]) + row, pol) : 0.0;
+      }
+      double* tile = s_tile[warp];
+#pragma unroll
+      for (int c = 0; c < 8; ++c) tile[c * kColStride + lane] = x[c];
+      __syncwarp();
+      const int c = lane & 7;
+      const bool i64 = (d.i64_mask >> ((c0 + c) & 31)) & 1u;
+#pragma unroll 1
+      for (int kk = 0; kk < 8; ++kk) {
+        const int r = 4 * kk + (lane >> 3);
+        const int g = __shfl_sync(0xffffffffu, gid, r);
+        long long img = 0;
+        const bool ok = base + r < p.nrows && g < gcap && c < nc &&
+                        distinct_image(tile[c * kColStride + r], i64, d.dropna, img);
+        distinct_insert(p, d, ok, (long long)g * p.vstride + c0 + c, img);
+      }
+      __syncwarp();
+    }
+  }
+}
+
+__global__ void gb_distinct_clear_kernel(DSlot* set, long long n) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    DSlot s;
+    s.entry = -1;
+    s.image = 0;
+    set[i] = s;
+  }
+}
+
+static int gb_distinct_launch(mb200_gb_table* t, const long long* keys, const void* const* vals, unsigned int i64_mask,
+                              int dropna, const long long* col_ids, const long long* images, long long nrows,
+                              cudaStream_t st) {
+  if (nrows == 0) return 0;
+  DevProps dp;
+  if (int rc = dev_props(&dp)) return rc;
+  const bool partial = col_ids != nullptr;
+  GbParams p = gb_params(t, keys, nrows);
+  DistinctParams d;
+  memset(&d, 0, sizeof(d));
+  d.set = t->dset;
+  d.mask = (unsigned long long)(t->dcap - 1);
+  d.col_ids = col_ids;
+  d.images = images;
+  d.i64_mask = i64_mask;
+  d.dropna = dropna ? 1 : 0;
+  if (!partial)
+    for (int c = 0; c < t->nvals; ++c) {
+      p.vals[c] = vals[c];
+      if (!p.vals[c]) return fail("mb200_gb_accumulate_distinct", "null value column");
+    }
+  return partial ? launch_direct(gb_distinct_kernel<true>, "gb_distinct_kernel", p, dp, st, d)
+                 : launch_direct(gb_distinct_kernel<false>, "gb_distinct_kernel", p, dp, st, d);
+}
+
+// emit_distinct: {rows, overflow} start from {ngroups, the table's overflow flag}
+__global__ void gb_distinct_count_init_kernel(const GbMeta* meta, long long ngroups, long long* out2) {
+  out2[0] = ngroups;
+  out2[1] = meta->overflow;
+}
+
+// one (key, -1, 0) row per group: the group's key is keys_by_gid[i] (dense: the i-th present key)
+__global__ void gb_distinct_group_rows_kernel(const long long* __restrict__ keys_by_gid, long long ngroups,
+                                              long long capacity, long long* out_keys, long long* out_cols,
+                                              long long* out_images, long long* out2) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= ngroups) return;
+  if (i >= capacity) {
+    out2[1] = 1;
+    return;
+  }
+  out_keys[i] = keys_by_gid[i];
+  out_cols[i] = -1;
+  out_images[i] = 0;
+}
+
+// one (key, column, image) row per occupied slot, appended after the group rows (one atomicAdd per warp)
+__global__ void __launch_bounds__(256) gb_distinct_entries_kernel(const DSlot* __restrict__ set, long long dcap,
+                                                                  int vstride, int dense, long long kbase,
+                                                                  const long long* __restrict__ keys_by_gid,
+                                                                  long long capacity, long long* out_keys,
+                                                                  long long* out_cols, long long* out_images,
+                                                                  long long* out2) {
+  const int lane = threadIdx.x & 31;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  // whole warps run every iteration: the trip count is rounded up to a multiple of 32 lanes' worth
+  const long long span = (dcap + 31) & ~31LL;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i - lane < span; i += stride) {
+    DSlot s;
+    s.entry = -1;
+    s.image = 0;
+    if (i < dcap) s = set[i];
+    const bool occ = s.entry >= 0;
+    const unsigned int m = __ballot_sync(0xffffffffu, occ);
+    if (!m) continue;
+    long long o = 0;
+    if (lane == __ffs(m) - 1) o = (long long)atomicAdd(reinterpret_cast<unsigned long long*>(out2), (unsigned long long)__popc(m));
+    o = __shfl_sync(0xffffffffu, o, __ffs(m) - 1) + __popc(m & ((1u << lane) - 1u));
+    if (!occ) continue;
+    if (o >= capacity) {
+      out2[1] = 1;
+      continue;
+    }
+    const long long g = s.entry / vstride;
+    out_keys[o] = dense ? kbase + g : keys_by_gid[g];
+    out_cols[o] = s.entry - g * vstride;
+    out_images[o] = s.image;
+  }
+}
 }  // namespace mb200
 
 using namespace mb200;
@@ -1756,6 +2009,8 @@ static int gb_create_impl(mb200_gb_table** table, int64_t group_capacity, int nv
   if ((flags & kGbArg) && flags != MB200_GB_ARGMIN && flags != MB200_GB_ARGMAX)
     return fail("mb200_gb_create", "ARGMIN / ARGMAX exclude every other flag");
   if ((flags & MB200_GB_VAR) && flags != kGbVarTable) return fail("mb200_gb_create", "a VAR table is SUM | COUNT | VAR");
+  if ((flags & MB200_GB_NUNIQUE) && flags != kGbNuniqueTable)
+    return fail("mb200_gb_create", "a NUNIQUE table is SIZE | NUNIQUE");
   DevProps dp;
   if (int rc = dev_props(&dp)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
@@ -1862,6 +2117,7 @@ extern "C" int mb200_gb_destroy(mb200_gb_table* t, mb200_stream_t stream) {
     if (t->present) cudaFreeAsync(t->present, st);
   }
   if (t->m2 && !t->arena) cudaFreeAsync(t->m2, st);
+  if (t->dset) cudaFreeAsync(t->dset, st);
   if (t->blockoff) cudaFreeAsync(t->blockoff, st);
   if (t->persisted) l2_carveout_release();  // the last table hands the carve-out back to normally managed L2
   delete t;
@@ -1884,6 +2140,8 @@ extern "C" int mb200_gb_accumulate(mb200_gb_table* t, const int64_t* keys, const
   if (nrows > 0 && !keys) return fail("mb200_gb_accumulate", "null keys");
   if (t->flags & kGbArg) return fail("mb200_gb_accumulate", "ARGMIN / ARGMAX tables take mb200_gb_accumulate_arg");
   if (t->m2_filled) return fail("mb200_gb_accumulate", "a VAR table takes no rows after mb200_gb_accumulate_m2");
+  if (t->distinct_filled)
+    return fail("mb200_gb_accumulate", "a NUNIQUE table takes no rows after mb200_gb_accumulate_distinct");
   if (int rc = gb_launch(t, reinterpret_cast<const long long*>(keys), vals, nullptr, nullptr, nrows, false,
                          (cudaStream_t)stream))
     return rc;
@@ -1899,6 +2157,8 @@ extern "C" int mb200_gb_merge_partial(mb200_gb_table* t, const int64_t* keys, co
   if (npartial > 0 && !keys) return fail("mb200_gb_merge_partial", "null keys");
   if (t->flags & kGbArg) return fail("mb200_gb_merge_partial", "ARGMIN / ARGMAX tables do not merge partial tables");
   if (t->m2_filled) return fail("mb200_gb_merge_partial", "a VAR table takes no rows after mb200_gb_accumulate_m2");
+  if (t->distinct_filled)
+    return fail("mb200_gb_merge_partial", "a NUNIQUE table takes no rows after mb200_gb_accumulate_distinct");
   return gb_launch(t, reinterpret_cast<const long long*>(keys), sums, cnts, reinterpret_cast<const long long*>(sizes),
                    npartial, true, (cudaStream_t)stream);
 }
@@ -1930,6 +2190,47 @@ extern "C" int mb200_gb_accumulate_m2(mb200_gb_table* t, const int64_t* keys, co
   if (int rc = gb_var_launch(t, reinterpret_cast<const long long*>(keys), vals, cnts, m2s, nrows, (cudaStream_t)stream))
     return rc;
   t->m2_filled = 1;
+  return 0;
+}
+
+extern "C" int mb200_gb_reserve_distinct(mb200_gb_table* t, int64_t capacity, mb200_stream_t stream) {
+  if (!t) return fail("mb200_gb_reserve_distinct", "null table");
+  if (!(t->flags & MB200_GB_NUNIQUE)) return fail("mb200_gb_reserve_distinct", "not a NUNIQUE table");
+  if (capacity < 1 || capacity > (1LL << 32) || (capacity & (capacity - 1)))
+    return fail("mb200_gb_reserve_distinct", "capacity must be a power of two in [1, 2^32]");
+  DevProps dp;
+  if (int rc = dev_props(&dp)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (t->dset_alloc < capacity) {
+    if (t->dset) cudaFreeAsync(t->dset, st);
+    t->dset = nullptr;
+    t->dset_alloc = t->dcap = 0;
+    MB_CUDA(cudaMallocAsync((void**)&t->dset, (size_t)capacity * sizeof(DSlot), st));
+    t->dset_alloc = capacity;
+  }
+  t->dcap = capacity;
+  long long grid = (capacity + 255) / 256;
+  if (grid > (long long)dp.sm_count * 8) grid = (long long)dp.sm_count * 8;
+  gb_distinct_clear_kernel<<<(unsigned)grid, 256, 0, st>>>(t->dset, capacity);
+  MB_LAUNCH_CHECK("gb_distinct_clear_kernel");
+  return 0;
+}
+
+extern "C" int mb200_gb_accumulate_distinct(mb200_gb_table* t, const int64_t* keys, const void* const* vals,
+                                            uint32_t i64_mask, int dropna, const int64_t* col_ids,
+                                            const int64_t* images, int64_t nrows, mb200_stream_t stream) {
+  if (!t) return fail("mb200_gb_accumulate_distinct", "null table");
+  if (!(t->flags & MB200_GB_NUNIQUE)) return fail("mb200_gb_accumulate_distinct", "not a NUNIQUE table");
+  if (!t->dset) return fail("mb200_gb_accumulate_distinct", "no distinct set: call mb200_gb_reserve_distinct first");
+  if (nrows < 0) return fail("mb200_gb_accumulate_distinct", "negative nrows");
+  if (nrows > 0 && !keys) return fail("mb200_gb_accumulate_distinct", "null keys");
+  if (nrows > 0 && col_ids && !images) return fail("mb200_gb_accumulate_distinct", "partial rows need an image column");
+  if (nrows > 0 && !col_ids && t->nvals > 0 && !vals) return fail("mb200_gb_accumulate_distinct", "null value columns");
+  if (int rc = gb_distinct_launch(t, reinterpret_cast<const long long*>(keys), vals, i64_mask, dropna,
+                                  reinterpret_cast<const long long*>(col_ids), reinterpret_cast<const long long*>(images),
+                                  nrows, (cudaStream_t)stream))
+    return rc;
+  t->distinct_filled = 1;
   return 0;
 }
 
@@ -2074,5 +2375,57 @@ static int gb_emit_impl(mb200_gb_table* t, int64_t ngroups, int sort, int64_t* o
   p.out_sizes = reinterpret_cast<long long*>(out_sizes);
   gb_emit_kernel<<<(unsigned)((ngroups + 255) / 256), 256, 0, st>>>(p);
   MB_LAUNCH_CHECK("gb_emit_kernel");
+  return 0;
+}
+
+extern "C" int mb200_gb_emit_distinct(mb200_gb_table* t, int64_t ngroups, int64_t capacity, int64_t* out_keys,
+                                      int64_t* out_cols, int64_t* out_images, void* scratch, int64_t* count_overflow_dev,
+                                      mb200_stream_t stream) {
+  if (!t) return fail("mb200_gb_emit_distinct", "null table");
+  if (!(t->flags & MB200_GB_NUNIQUE) || !t->dset) return fail("mb200_gb_emit_distinct", "not a NUNIQUE table with a set");
+  if (ngroups < 0 || ngroups > t->gcap) return fail("mb200_gb_emit_distinct", "ngroups out of range");
+  if (capacity < 0) return fail("mb200_gb_emit_distinct", "negative capacity");
+  if (!count_overflow_dev) return fail("mb200_gb_emit_distinct", "null count output");
+  if (capacity > 0 && (!out_keys || !out_cols || !out_images)) return fail("mb200_gb_emit_distinct", "null output");
+  if (!scratch) return fail("mb200_gb_emit_distinct", "null scratch");
+  DevProps dp;
+  if (int rc = dev_props(&dp)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  char* s = static_cast<char*>(scratch);
+  long long* keys_by_gid = reinterpret_cast<long long*>(s);
+  long long* perm = reinterpret_cast<long long*>(s + (size_t)(ngroups > 0 ? ngroups : 1) * 8);
+  long long* out2 = reinterpret_cast<long long*>(count_overflow_dev);
+  if (ngroups > 0) {
+    if (t->dense) {  // the present keys, ascending (as gb_emit_impl lists them)
+      if (int rc = dense_finalize_presence(t, st)) return rc;
+      const long long w0 = t->win_lo / 4, nw = (t->win_hi - t->win_lo + 3) / 4;
+      const long long nblocks = nw > 0 ? (nw + 255) / 256 : 1;
+      dense_count_kernel<<<(unsigned)nblocks, 256, 0, st>>>(t->present + w0, nw, t->blockoff);
+      MB_LAUNCH_CHECK("dense_count_kernel");
+      dense_scan_kernel<<<1, 1024, 0, st>>>(t->blockoff, nblocks, t->meta);
+      MB_LAUNCH_CHECK("dense_scan_kernel");
+      dense_fill_kernel<<<(unsigned)nblocks, 256, 0, st>>>(t->present + w0, nw, t->blockoff, t->kbase, t->win_lo,
+                                                          keys_by_gid, perm, ngroups);
+      MB_LAUNCH_CHECK("dense_fill_kernel");
+    } else {  // key of every group id
+      gb_collect_kernel<<<(unsigned)((t->cap + 255) / 256), 256, 0, st>>>(t->slots, t->cap, t->gcap, keys_by_gid, perm,
+                                                                          t->meta);
+      MB_LAUNCH_CHECK("gb_collect_kernel");
+    }
+  }
+  gb_distinct_count_init_kernel<<<1, 1, 0, st>>>(t->meta, ngroups, out2);
+  MB_LAUNCH_CHECK("gb_distinct_count_init_kernel");
+  if (ngroups > 0) {
+    gb_distinct_group_rows_kernel<<<(unsigned)((ngroups + 255) / 256), 256, 0, st>>>(
+        keys_by_gid, ngroups, capacity, reinterpret_cast<long long*>(out_keys), reinterpret_cast<long long*>(out_cols),
+        reinterpret_cast<long long*>(out_images), out2);
+    MB_LAUNCH_CHECK("gb_distinct_group_rows_kernel");
+  }
+  long long grid = (t->dcap + 255) / 256;
+  if (grid > (long long)dp.sm_count * 8) grid = (long long)dp.sm_count * 8;
+  gb_distinct_entries_kernel<<<(unsigned)grid, 256, 0, st>>>(
+      t->dset, t->dcap, t->vstride, t->dense, t->kbase, keys_by_gid, capacity, reinterpret_cast<long long*>(out_keys),
+      reinterpret_cast<long long*>(out_cols), reinterpret_cast<long long*>(out_images), out2);
+  MB_LAUNCH_CHECK("gb_distinct_entries_kernel");
   return 0;
 }

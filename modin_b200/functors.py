@@ -1653,6 +1653,153 @@ def fused_dense_groupby(map_fn: "DevGroupbyMap", reduce_fn: "DevGroupbyReduce", 
     return _finished_block(agg, keys, key_label, _partial_cols(agg, sums, cnts, sizes), labels)
 
 
+# ------------------------------------------------------------------ groupby.nunique
+# Modin runs nunique as a full-axis groupby, not as GroupByReduce: distinct counts do not merge element-wise, so neither
+# the partial tables of ``DevGroupbyReduce`` nor ``fused_dense_groupby`` apply.  One NUNIQUE table per GPU takes every
+# row partition resident on it: pass 1 inserts the groups, pass 2 inserts one (group, column, value) entry per value into
+# the table's distinct set and counts the new ones.
+_NUNIQUE = _lib.GB_SIZE | _lib.GB_NUNIQUE
+
+
+def _next_pow2(n: int) -> int:
+    return 1 << max(int(n) - 1, 0).bit_length()
+
+
+def distinct_batches(rows: int, ncols: int):
+    """The column batches ``[lo, hi)`` of ``groupby.nunique`` over ``rows`` rows: at most MAX_COLS columns each, whose
+    distinct set -- ``next_pow2(2 * rows * width)`` slots of 16 bytes, so at most half full -- fits in
+    ``GroupbyDistinctBytes``; one column at least, whatever its set costs.  A function of ``rows`` and ``ncols`` alone,
+    so ranks that plan on the same numbers run the same batches."""
+    from .config import GroupbyDistinctBytes
+
+    budget = GroupbyDistinctBytes.get()
+    out, lo = [], 0
+    while lo < ncols:
+        w = 1
+        while lo + w < ncols and w < _lib.MAX_COLS and 16 * _next_pow2(2 * rows * (w + 1)) <= budget:
+            w += 1
+        out.append((lo, lo + w))
+        lo += w
+    return out
+
+
+def _distinct_table(keys, nvals: int, capacity_hint: int, partial: bool = False):
+    """A NUNIQUE table of ``nvals`` value columns holding the groups of the key columns ``keys`` (pass 1), dense or
+    hashed as ``plan_table`` decides; a hash table is grown until it holds every group.  Returns (table, groups)."""
+    plan = ops.plan_table(keys, nvals, _NUNIQUE, capacity_hint, partial=partial)
+    cap = plan.capacity
+    while True:
+        table = plan.create(cap)
+        for k in keys:
+            table.accumulate(k, [])
+        ng, overflow = table.ngroups()
+        if not overflow or table.kbase is not None:
+            ops.refuse_dense_overflow((ng, overflow))
+            return table, ng
+        table.close()
+        if cap >= max(plan.rows, 1024):
+            raise _lib.B200Error("group table overflow even with capacity == number of rows")
+        cap = min(max(cap * 4, 1024), max(plan.rows, 1024))
+
+
+def _distinct_filled(table, entries: int, inputs):
+    """Pass 2: a distinct set for ``entries`` values at most, then every input ``(keys, vals | None, col_ids, images,
+    dropna)``.  Raises when the set filled up, so that no count is ever short."""
+    table.reserve_distinct(_next_pow2(2 * max(entries, 1)))
+    for keys, vals, col_ids, images, dropna in inputs:
+        table.accumulate_distinct(keys, vals, dropna=dropna, col_ids=col_ids, images=images)
+    ng, overflow = table.ngroups()
+    if overflow:
+        raise _lib.B200Error("groupby.nunique: the distinct set is full")
+    return ng
+
+
+def groupby_nunique(blocks, by_blocks, labels, dropna: bool = True, capacity_hint: int = 1 << 20):
+    """``df.groupby(key).nunique(dropna)`` over this rank's row blocks and their key blocks (one int64 key column each;
+    ``labels``: the frame's column labels).  Returns the result block: ascending group keys, one int64 column of
+    distinct counts per value column (float64, int64, or bool widened to int64).
+
+    One process: per column batch (``distinct_batches``), one table takes every row block and emits its counts.
+    Across ranks every rank emits its tables' distinct sets instead -- one ``(key, -1, 0)`` row per group, so that a
+    group without values still reaches the result, and one ``(key, column, image)`` row per entry -- sorts them by key
+    and sends them in ONE ``dist.exchange_by_key_range`` (24 bytes per entry), then counts the key range it received
+    with one table per batch.  A rank without rows takes part in every collective."""
+    from . import dist
+
+    key_label = by_blocks[0].columns[0]
+    _, vlabels = _value_positions(pandas.Index(labels), key_label)
+    keys, vals = [], []
+    for block, by_block in zip(blocks, by_blocks):
+        k, _, v, _ = _split_key_values(block, by_block, "groupby_nunique")
+        if any(c.dtype not in (np.float64, np.int64, np.bool_) for c in v):
+            raise NotImplementedError("device groupby.nunique counts float64, int64 and bool columns")
+        keys.append(k)
+        vals.append(ops.cast_columns_i64(v))
+    W = len(vlabels)
+    rows = sum(len(k) for k in keys)
+    spans = dist.is_distributed() and not all(getattr(b, "replicated", False) for b in blocks)
+    # ranks plan their batches on the job's row count: every rank then runs the same batches, and no rank receives
+    # more entries per batch than the job has values
+    batches = distinct_batches(dist.control_sum(rows) if spans else rows, W) or [(0, 0)]
+    if not spans:
+        out_keys, counts = None, []
+        for lo, hi in batches:
+            table, _ = _distinct_table(keys, hi - lo, capacity_hint)
+            try:
+                ng = _distinct_filled(table, rows * (hi - lo), [(k, v[lo:hi], None, None, dropna) for k, v in zip(keys, vals)])
+                k_out, _, cnts, _ = table.emit(ng, sort=True)
+            finally:
+                table.close()
+            out_keys = k_out
+            counts += cnts or []
+        return _group_block(counts, vlabels, out_keys, key_label)
+    return _nunique_across_ranks(keys, vals, batches, dropna, capacity_hint, vlabels, key_label)
+
+
+def _nunique_across_ranks(keys, vals, batches, dropna, capacity_hint, vlabels, key_label):
+    from . import dist
+
+    rows = sum(len(k) for k in keys)
+    sent_k, sent_c, sent_i = [], [], []
+    for lo, hi in batches:
+        table, ng = _distinct_table(keys, hi - lo, capacity_hint)
+        try:
+            _distinct_filled(table, rows * (hi - lo), [(k, v[lo:hi], None, None, dropna) for k, v in zip(keys, vals)])
+            k, c, i, count = table.emit_distinct(ng, ng + rows * (hi - lo))
+            n, overflow = count.tolist()
+        finally:
+            table.close()
+        if overflow:
+            raise _lib.B200Error("groupby.nunique: more distinct entries than the emit has room for")
+        # the emit's first ng rows are its (key, -1, 0) group rows: the first batch sends them, the others send their
+        # entries only, with the column ids of the whole frame, so that one exchange serves every batch
+        first = 0 if lo == 0 else ng
+        cut = lambda col: DeviceColumn(col.data[first:n], np.int64)  # noqa: E731
+        sent_k.append(cut(k))
+        sent_c.append(ops.map_columns("add_s", [cut(c)], s0=[lo])[0] if lo else cut(c))
+        sent_i.append(cut(i))
+    # one table of every batch's rows, sorted by key in place (the emits' buffers are this function's), then ONE exchange
+    sk = ops.concat_columns(sent_k)
+    perm = ops.iota(0, len(sk))
+    ops.sort_pairs(sk, perm)
+    sc, si = ops.take_columns([ops.concat_columns(sent_c), ops.concat_columns(sent_i)], perm)
+    rk, (rc, ri) = dist.exchange_by_key_range(sk.data, [sc.data, si.data])
+    rkeys, rcols, rimgs = DeviceColumn(rk, np.int64), DeviceColumn(rc, np.int64), DeviceColumn(ri, np.int64)
+    out_keys, counts = None, []
+    for lo, hi in batches:
+        # the batch's column ids start at 0; rows of other batches fall outside [0, hi - lo) and add nothing
+        bcols = ops.map_columns("sub_s", [rcols], s0=[lo])[0] if lo else rcols
+        table, _ = _distinct_table([rkeys], hi - lo, len(rkeys), partial=True)
+        try:
+            ng = _distinct_filled(table, len(rkeys), [(rkeys, None, bcols, rimgs, True)])
+            k_out, _, cnts, _ = table.emit(ng, sort=True)
+        finally:
+            table.close()
+        out_keys = k_out
+        counts += cnts or []
+    return _group_block(counts, vlabels, out_keys, key_label)
+
+
 # ------------------------------------------------------------------ broadcast merge functor
 _BOOL_MISSES = "device merge(how='left') with a bool payload column and unmatched left rows (pandas gives object dtype)"
 

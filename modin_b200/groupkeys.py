@@ -149,7 +149,7 @@ def restore_keys(blocks: List[DeviceBlock], image, dropna: bool = True, names=No
 
 
 # ---- dictionary aggregation --------------------------------------------------------------------------------------
-_DICT_AGGS = ("sum", "count", "mean", "min", "max", "first", "last", "idxmax", "idxmin", "var", "std")
+_DICT_AGGS = ("sum", "count", "mean", "min", "max", "first", "last", "idxmax", "idxmin", "var", "std", "nunique")
 
 
 def split_aggregations(spec: dict, columns, keys=()) -> Dict[str, list]:

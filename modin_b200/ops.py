@@ -258,7 +258,7 @@ def arg_reduce_columns(op: str, cols: Sequence[DeviceColumn], variant: int = 0):
 _GB_ARG = _lib.GB_ARGMIN | _lib.GB_ARGMAX  # idxmin / idxmax: extreme images in ``cnt``, row positions in ``acc``
 _GB_POS = _lib.GB_FIRST | _lib.GB_LAST | _GB_ARG  # tables of int64 row positions (first / last / idxmin / idxmax)
 _GB_ACC = _lib.GB_SUM | _lib.GB_MIN | _lib.GB_MAX | _GB_POS
-_GB_CNT = _lib.GB_COUNT | _GB_ARG  # tables with a ``cnt`` array
+_GB_CNT = _lib.GB_COUNT | _GB_ARG | _lib.GB_NUNIQUE  # tables with a ``cnt`` array (a NUNIQUE table's distinct counts)
 _DENSE_ARRAYS = ("acc", "cnt", "size", "present")
 
 
@@ -389,6 +389,38 @@ class GroupTable:
             _lib.check(self.lib.mb200_gb_accumulate_m2(self.handle, keys.ptr, ptrs(vals), ptrs(cnts), ptrs(m2s), len(keys),
                                                        current_stream()))  # fmt: skip
 
+    def reserve_distinct(self, capacity: int):
+        """Give a nunique table a distinct set of ``capacity`` (a power of two) 16-byte slots, or clear the one it has
+        (mb200_gb_reserve_distinct)."""
+        _lib.check(self.lib.mb200_gb_reserve_distinct(self.handle, int(capacity), current_stream()))
+
+    def accumulate_distinct(self, keys: DeviceColumn, vals=None, dropna: bool = True, col_ids=None, images=None):
+        """Pass 2 of a nunique table (mb200_gb_accumulate_distinct), after every pass-1 call: raw float64 / int64 rows
+        ``vals`` (NaN skipped under ``dropna``), or the ``(col_ids, images)`` rows of other tables' ``emit_distinct``.
+        Every (group, column, value) not in the set yet adds 1 to the group's count of that column."""
+        if col_ids is None:
+            if any(v.dtype not in (np.float64, np.int64) for v in vals):
+                raise TypeError("device groupby.nunique takes float64 and int64 value columns (bool widened to int64)")
+            mask = sum(1 << j for j, v in enumerate(vals) if v.dtype == np.int64)
+            ptrs = _lib.ptr_array([v.ptr for v in vals]) if vals else None
+            args = (ptrs, mask, 1 if dropna else 0, None, None)
+        else:
+            args = (None, 0, 1 if dropna else 0, col_ids.ptr, images.ptr)
+        with _timed("gb_accumulate_distinct"):
+            _lib.check(self.lib.mb200_gb_accumulate_distinct(self.handle, keys.ptr, *args, len(keys), current_stream()))
+
+    def emit_distinct(self, ngroups: int, capacity: int):
+        """The distinct set as ``(keys, col_ids, images, count_dev)`` rows for another nunique table's partial pass 2:
+        one ``(key, -1, 0)`` row per group, then one row per entry, valid up to ``count_dev[0]`` (device int64[2]
+        ``{rows, overflow}``; mb200_gb_emit_distinct)."""
+        t = torch_mod()
+        keys, cols, imgs = (DeviceColumn.empty(capacity, np.int64) for _ in range(3))
+        count = t.empty(2, dtype=t.int64, device=current_device())
+        scratch = _scratch(self.lib.mb200_gb_emit_scratch_bytes(ngroups), "gb_emit")
+        _lib.check(self.lib.mb200_gb_emit_distinct(self.handle, int(ngroups), int(capacity), keys.ptr, cols.ptr, imgs.ptr,
+                                                   scratch.data_ptr(), count.data_ptr(), current_stream()))  # fmt: skip
+        return keys, cols, imgs, count
+
     def merge_partial(self, keys: DeviceColumn, sums, cnts=None, sizes: Optional[DeviceColumn] = None):
         ps = _lib.ptr_array([v.ptr for v in sums]) if sums else None
         pc = _lib.ptr_array([v.ptr for v in cnts]) if cnts else None
@@ -408,7 +440,7 @@ class GroupTable:
         acc_dtype = np.int64 if self.flags & _GB_POS else np.float64  # first / last / idxmin / idxmax emit row positions
         nsums = 2 * self.nvals if self.flags & _lib.GB_VAR else self.nvals  # var / std: the sums, then the M2s
         sums = [DeviceColumn.empty(rows, acc_dtype) for _ in range(nsums)] if self.flags & _GB_ACC else None
-        cnts = [DeviceColumn.empty(rows, np.int64) for _ in range(self.nvals)] if self.flags & _lib.GB_COUNT else None
+        cnts = [DeviceColumn.empty(rows, np.int64) for _ in range(self.nvals)] if self.flags & _GB_CNT & ~_GB_ARG else None
         sizes = DeviceColumn.empty(rows, np.int64) if self.flags & _lib.GB_SIZE else None
         return DeviceColumn.empty(rows, np.int64), sums, cnts, sizes
 

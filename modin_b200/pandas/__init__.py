@@ -647,12 +647,17 @@ class DataFrameGroupBy:
             raise NotImplementedError(f"groupby.std(engine={engine!r}) is not on the B200 path")
         return self._wrap_aggregation(type(self._query_compiler).groupby_std, numeric_only, agg_kwargs=dict(ddof=ddof))
 
+    def nunique(self, dropna=True):
+        """The number of distinct values of every column per group (int64; NaN left out under ``dropna``, else counted
+        once), passed on as modin/pandas/groupby.py:1399-1406 does."""
+        return self._wrap_aggregation(type(self._query_compiler).groupby_nunique, agg_kwargs=dict(dropna=dropna))
+
     def size(self):
         res = self._wrap_aggregation(type(self._query_compiler).groupby_size)
         return Series(query_compiler=res._query_compiler)
 
     def agg(self, func, *args, **kwargs):
-        if isinstance(func, str) and func in ("var", "std") and not args:
+        if isinstance(func, str) and func in ("var", "std", "nunique") and not args:
             return getattr(self, func)(**kwargs)
         if isinstance(func, str) and func in ("sum", "count", "mean", "size", "min", "max", "first", "last", "idxmax",
                                                  "idxmin"):

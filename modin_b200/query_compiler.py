@@ -45,6 +45,7 @@ from .functors import (
     DevReduce,
     DevRound,
     DevVar,
+    groupby_nunique,
 )
 
 
@@ -102,12 +103,37 @@ def _var_ddof(agg: str, agg_kwargs):
     return int(ddof)  # pandas 3.0.2's group_var takes ddof as an integer: 1.5 acts as 1, -0.5 as 0
 
 
+def _nunique_dropna(agg_kwargs) -> bool:
+    """``dropna`` of ``groupby.nunique`` from the ``agg_kwargs`` Modin passes (modin/pandas/groupby.py:1399-1406): whether
+    NaN is left out of the count.  Any other argument is refused."""
+    kw = dict(agg_kwargs or {})
+    dropna = kw.pop("dropna", True)
+    if kw:
+        raise NotImplementedError(f"groupby.nunique({', '.join(kw)}=) is not on the B200 path")
+    if not isinstance(dropna, (bool, np.bool_)):
+        raise ValueError(f"dropna must be a boolean, got {dropna!r}")
+    return bool(dropna)
+
+
+def _nunique_frame(frame, by_frame, dropna: bool):
+    """``groupby.nunique`` of ``frame`` by the one int64 key column of ``by_frame`` (``functors.groupby_nunique``): a
+    frame of one row block.  It is not a GroupByReduce: distinct counts do not merge as partial tables."""
+    blocks = [concat_cols([p.get() for p in row]) if len(row) > 1 else row[0].get() for row in frame._partitions]
+    by_blocks = [row[0].get() for row in by_frame._partitions]
+    if [b.nrows for b in blocks] != [b.nrows for b in by_blocks]:
+        raise NotImplementedError("group keys partitioned unlike the frame's rows are not on the B200 path")
+    block = groupby_nunique(blocks, by_blocks, frame.columns, dropna)
+    pc = frame._partition_mgr_cls._partition_class
+    return type(frame)(np.array([[pc(block)]], dtype=object), None, None, None, None)
+
+
 def _groupby_reduce(agg: str):
     """``qc.groupby_<agg>`` (qc.py:3741-3748, alg/groupby.py) over device blocks.  ``by`` is a query compiler of key
     columns with the frame's rows; ``key_names`` replaces the names of the result's keys (``groupby(level=)``).
-    ``agg_kwargs`` are read by first / last (``skipna``, ``min_count``), idxmax / idxmin (``skipna``, ``axis``) and
-    var / std (``ddof``) only; the other aggregations ignore them."""
-    map_f, red_f = DevGroupbyMap(agg), DevGroupbyReduce(agg)
+    ``agg_kwargs`` are read by first / last (``skipna``, ``min_count``), idxmax / idxmin (``skipna``, ``axis``), var /
+    std (``ddof``) and nunique (``dropna``) only; the other aggregations ignore them.  nunique is not a GroupByReduce:
+    it runs ``_nunique_frame``."""
+    map_f, red_f = (DevGroupbyMap(agg), DevGroupbyReduce(agg)) if agg != "nunique" else (None, None)
 
     def caller(query_compiler, by, axis, groupby_kwargs, agg_args, agg_kwargs, drop=False, key_names=None, **kwargs):
         if by is None and groupby_kwargs.get("level") is not None and hasattr(query_compiler, "_b200_level_key"):
@@ -124,6 +150,8 @@ def _groupby_reduce(agg: str):
             _arg_agg_kwargs(agg, agg_kwargs)
         if agg in ("var", "std"):
             fns = (map_f, DevGroupbyReduce(agg, ddof=_var_ddof(agg, agg_kwargs)))
+        if agg == "nunique":
+            dropna = _nunique_dropna(agg_kwargs)
         frame, by_frame = query_compiler._modin_frame, by._modin_frame
         # a float64 key or several int64 keys: the single-key groupby runs on their int64 image and the G result keys
         # are restored afterwards (groupkeys.py); one int64 key is its own image
@@ -144,7 +172,10 @@ def _groupby_reduce(agg: str):
             fns = (DevGroupbyMap(agg, label_dtype=labels), DevGroupbyReduce(agg, nan_key=nan_key))
         # the functors themselves, not lambdas around them: the partition manager recognises them and fuses map +
         # reduce into one direct-addressed table per GPU when the key range allows (pm.groupby_reduce)
-        new_frame = frame.groupby_reduce(axis, by_frame, *fns)
+        if agg == "nunique":
+            new_frame = _nunique_frame(frame, by_frame, dropna)
+        else:
+            new_frame = frame.groupby_reduce(axis, by_frame, *fns)
         if image is not None or key_names is not None:
             blocks = gk.restore_keys([row[0].get() for row in new_frame._partitions], image,
                                      groupby_kwargs.get("dropna", True), key_names)  # fmt: skip
@@ -260,9 +291,11 @@ def device_operations(alg):
         groupby_idxmin = _groupby_reduce("idxmin")
         groupby_var = _groupby_reduce("var")
         groupby_std = _groupby_reduce("std")
+        groupby_nunique = _groupby_reduce("nunique")  # a full-axis groupby, as in Modin (qc.groupby_nunique)
 
-        _DEVICE_AGGS = ("sum", "count", "size", "mean", "min", "max", "first", "last", "idxmax", "idxmin", "var", "std")
-        _KWARG_AGGS = ("first", "last", "idxmax", "idxmin", "var", "std")  # aggregations that read agg_kwargs
+        _DEVICE_AGGS = ("sum", "count", "size", "mean", "min", "max", "first", "last", "idxmax", "idxmin", "var", "std",
+                        "nunique")  # fmt: skip
+        _KWARG_AGGS = ("first", "last", "idxmax", "idxmin", "var", "std", "nunique")  # aggregations that read agg_kwargs
 
         def groupby_agg(self, by, agg_func, axis, groupby_kwargs, agg_args, agg_kwargs, how="axis_wise", drop=False,
                         series_groupby=False):  # fmt: skip
@@ -285,12 +318,12 @@ def device_operations(alg):
                 raise NotImplementedError("device groupby: key columns of the same frame, axis=0")
             spec = {col: fn[0] if isinstance(fn, (list, tuple)) and len(fn) == 1 else fn for col, fn in agg_func.items()}
             by_func = gk.split_aggregations(spec, self.columns, set(by.columns) if drop else ())
-            if len(by_func) > 1 and set(by_func) & {"first", "last", "idxmax", "idxmin", "var", "std"} \
+            if len(by_func) > 1 and set(by_func) & {"first", "last", "idxmax", "idxmin", "var", "std", "nunique"} \
                     and dist.is_distributed():  # fmt: skip
                 # across ranks the fused dense path of the other functions and the key-range exchange of first / last /
-                # idxmax / idxmin / var / std give each rank a different key range
-                raise NotImplementedError("groupby.agg mixing first / last / idxmax / idxmin / var / std with other "
-                                          "functions across ranks")  # fmt: skip
+                # idxmax / idxmin / var / std / nunique give each rank a different key range
+                raise NotImplementedError("groupby.agg mixing first / last / idxmax / idxmin / var / std / nunique with "
+                                          "other functions across ranks")  # fmt: skip
             if any(isinstance(fn, (list, tuple)) for fn in agg_func.values()):
                 raise NotImplementedError("groupby.agg with lists of functions (two-level result columns)")
             kw = dict(groupby_kwargs, as_index=True)
